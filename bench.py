@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- ray-samples/s of the per-ray rendering hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
                     [--workload black_800|black_400|cfg1|fern_high|train_dtu] [--shard images|rays]
 
 Headline (default flags): a "step" renders ONE full synthetic query image through the hot path (sample_depth -> coarse
@@ -22,9 +22,8 @@ Other BASELINE.json configurations (selectable as the main line with --workload,
   train_dtu  cfg5: one optimisation step per rank on 512 rays of a DTU-shape scene (8 views 304x400), native backward,
              flat-bucket gradient all-reduce (timed separately), Adam = weak scaling
 
---impl reference times the UNMODIFIED reference's own implementation of the path (baseline/_ref, the verbatim copy made by
-baseline/install_ref.py: NeuralRayBaseRenderer.render_impl over the chunk loop of renderer.py:237-254, encoder outputs
-given) on the box's host cores; when the copy is absent it falls back to the oracle port and says so (`kind`).
+--impl reference times the oracle port of the reference's PyTorch path (oracle/neuray_oracle.py: render_impl over the chunk
+loop of the reference's renderer.py:237-254, encoder outputs given) on the host cores (`kind` = "port").
 """
 import argparse
 import json
@@ -319,11 +318,9 @@ def train_step_bench(ctx, steps, warmup, e2e=True):
 # ---- reference arm / CPU baselines ------------------------------------------------------------------------------------------
 
 def _load_reference():
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import ref_import
-    if not ref_import.available():
-        return None
-    return ref_import.load_reference()
+    """The reference's sources are not part of the project, so the arms that would run them report the oracle port
+    (cpu_baseline) or "unavailable" instead."""
+    return None
 
 
 def reference_net(ref_mod, cfg, seed=0, device="cpu"):
@@ -353,7 +350,7 @@ def reference_render_chunks(net, que, ref, ray_batch_num):
 
 def cpu_arm(wl_name, n_rays, steps, warmup, threads=None):
     """ray-samples/s of the reference's CPU implementation on `n_rays` rays of the workload (same maps, same weights).
-    Returns (value, seconds per pass, kind, threads).  kind = "reference" (baseline/_ref) or "port" (oracle)."""
+    Returns (value, seconds per pass, kind, threads).  kind = "port" (oracle)."""
     from neuray_b200 import synthetic, renderer
     wl = WORKLOADS[wl_name]
     dn_c, dn_f = wl["dn"]
@@ -414,8 +411,7 @@ def run_reference(args):
     n_rays = args.ref_rays
     v, t, kind, threads = cpu_arm(args.workload, n_rays, args.steps, max(1, min(args.warmup, 1)))
     sample = f"{n_rays} rays x ({dn_c}+{dn_f}) samples of the workload per step (a contiguous stretch of image rows)"
-    what = ("the UNMODIFIED reference (baseline/_ref): NeuralRayBaseRenderer.render_impl over render()'s chunk loop, encoder outputs given"
-            if kind == "reference" else "oracle port of the reference's PyTorch path (baseline/_ref missing)")
+    what = "oracle port of the reference's PyTorch path: render_impl over render()'s chunk loop, encoder outputs given"
     line = {
         "impl": "reference", "metric": METRIC, "value": v, "unit": "ray-samples/s", "n_gpus": args.gpus, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -429,10 +425,10 @@ def run_reference(args):
 
 def eager_gpu_baseline(dq, dr, cfg, dn, dev, rays=4096, reps=3):
     """GPU-vs-GPU baseline (SURVEY.md 8d): the UNMODIFIED reference's own render_impl (coarse + fine pass) as PyTorch-eager
-    CUDA ops on the same B200, on one 4096-ray chunk (render.py's default chunk) of the same workload and weights."""
+    CUDA ops on the same GPU, on one 4096-ray chunk (render.py's default chunk) of the same workload and weights."""
     ref_mod = _load_reference()
     if ref_mod is None:
-        return {"unavailable": "baseline/_ref missing (run baseline/install_ref.py before gpurun)"}
+        return {"unavailable": "the reference's sources are not part of the project"}
     net = reference_net(ref_mod, cfg, device=dev)
     n = dq["coords"].shape[1]
     start = max(0, n // 2 - rays // 2)                 # a stretch of rays through the middle of the image
@@ -514,7 +510,7 @@ def encoders_bench(dr, dev, reps=5):
            "what": "image_encoder + vis_encoder of all reference views into the channel-last frame pack (3xTF32 tensor-core convolutions: fp32 accuracy)"}
     ref_mod = _load_reference()
     if ref_mod is None:
-        res["reference"] = {"unavailable": "baseline/_ref missing"}
+        res["reference"] = {"unavailable": "the reference's sources are not part of the project"}
         return res
     from network.ops import ResUNetLight
     from network.vis_encoder import DefaultVisEncoder
@@ -673,7 +669,10 @@ def run_headline(ctx, args):
     # ---- device-resident arm (value) with per-kernel event timing of the two kernels of a pass ----
     dq = {k: v.to(dev) for k, v in que.items()}
     dr = {k: v.to(dev) for k, v in ref.items()}
-    step_resident = lambda: step_device(dict(dq), dr)      # the per-frame map repack runs inside every render() call
+    last = {}
+
+    def step_resident():      # the per-frame map repack runs inside every render() call
+        last["out"] = step_device(dict(dq), dr)
 
     sampler = ClockSampler(ctx.local)
     for _ in range(args.warmup):
@@ -690,6 +689,8 @@ def run_headline(ctx, args):
     rk_ms = [b.elapsed_time(c) for _, b, _, c in prof]
     pk_samples = [n for _, _, n, _ in prof]
     value = world * samples_per_step * args.steps / t_res
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {k: last["out"][k] for k in out_keys})
 
     # ---- end-to-end arm ----
     t_e2e = ctx.timed(step_e2e, args.steps, args.warmup)
@@ -721,8 +722,8 @@ def run_headline(ctx, args):
     if os.path.exists(pth):
         peaks = json.load(open(pth))
         peaks_src = "measured"
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)      # kernel timed inside a long step -> sustained figure
-    peak_hbm = peaks.get("hbm_gbs", 6650.0)
+    peak_tf = peaks.get("tf32_tflops_sustained", 495.0)       # H100 SXM data sheet, dense TF32 (700 W card) when not measured: the kernel's wgmma are TF32
+    peak_hbm = peaks.get("hbm_gbs", 3350.0)
     fl = point_kernel_flops_per_sample(rfn, False)
     pk_time = sum(pk_ms) / 1e3
     achieved_tf = sum(pk_samples) * fl / pk_time / 1e12
@@ -751,7 +752,7 @@ def run_headline(ctx, args):
         "config": {"workload": wl["desc"], "rays_per_image": rays, "images_per_step_per_gpu": 1, "ray_batch_num": args.ray_batch,
                    "parallelism": f"one image per rank x{world}" + (", NCCL all-gather of rendered tiles" if world > 1 else ""),
                    "e2e_pipeline": "inputs of step i+1 are uploaded on a copy stream while step i renders",
-                   "l2": "inputs (143 MB of maps at black_800) exceed the 126 MB L2; no explicit flush"},
+                   "l2": "inputs (143 MB of maps at black_800) exceed the 50 MB L2; no explicit flush"},
         "per_gpu": value / world,
         "e2e": {"value": e2e_value, "unit": "ray-samples/s", "h2d_bytes_per_step": up_bytes(que, ref), "d2h_bytes_per_step": d2h,
                 "ms_per_step": t_e2e / args.steps * 1e3},
@@ -759,10 +760,10 @@ def run_headline(ctx, args):
         "clocks": sampler.summary(),
         "roofline": {"bound": "tensor", "kernel": "nr::pkt::pm3::point_kernel_pm3", "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s",
                      "frac": achieved_tf / peak_tf, "traffic": traffic, "traffic_unit": "DRAM bytes per launch (ncu --set full)",
-                     "traffic_source": traffic_src, "peak_source": f"{peaks_src} bf16_tflops_sustained",
+                     "traffic_source": traffic_src, "peak_source": ("measured" if "tf32_tflops_sustained" in peaks else "H100 SXM data sheet") + " tf32_tflops_sustained",
                      "flops_per_ray_sample": fl, "launches": n_launch, "avg_launch_ms": sum(pk_ms) / max(n_launch, 1),
                      "share_of_step": pk_time / t_res, "ray_kernel_share_of_step": sum(rk_ms) / 1e3 / t_res,
-                     "note": "dense layers on tcgen05 with 3xTF32 (3 MMAs per algorithmic one)"},
+                     "note": "dense layers on wgmma with 3xTF32 (3 MMAs per algorithmic one)"},
         "roofline_gather": {"bound": "hbm", "achieved": gather_gbs, "peak": peak_hbm, "unit": "GB/s", "frac": gather_gbs / peak_hbm,
                             "bytes_per_ray_sample": rfn * 1072,
                             "note": "gather runs inside the point kernel; algorithmic bytes / point-kernel time"},
@@ -799,6 +800,15 @@ def run_headline(ctx, args):
     print(json.dumps(line))
 
 
+def dump_outputs(dirname, outs):
+    """What the timed path returned in its last step, one float32 DIR/<name>.npy per output, so that two builds can be
+    compared output for output (the inputs are seeded)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    for k, v in outs.items():
+        np.save(os.path.join(dirname, f"{k}.npy"), v.detach().float().cpu().numpy())
+
+
 def up_bytes(que, ref):
     return sum(v.numel() * v.element_size() for d in (que, ref) for v in d.values())
 
@@ -832,7 +842,12 @@ def main():
     ap.add_argument("--ref-rays", type=int, default=512, help="rays per step for --impl reference")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-aux", action="store_true", help="skip the auxiliary legs (fern_high sharded, train_dtu, eager GPU baseline)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of the headline workloads (black_800, black_400, cfg1) as "
+                         "DIR/<name>.npy (float32): pixel_colors_nr, pixel_colors_nr_fine, render_depth_fine, ray_mask_fine")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.workload in ("fern_high", "train_dtu")):
+        ap.error("--dump-outputs is implemented for the headline workloads of --impl b200 only")
     if args.impl == "reference":
         if args.workload in ("fern_high", "train_dtu"):
             args.workload = "fern_high" if args.workload == "fern_high" else "black_800"

@@ -13,7 +13,7 @@
  *   - every call is enqueued on `stream` (a cudaStream_t passed as void*) and never synchronises the host
  *   - returns 0 on success, a negative NR_E_* code on failure; nr_last_error() gives a thread-local message
  *   - one query view per call (qn == 1), exactly like every call site in the reference
- *   - sm_100a only; there is no CPU fallback
+ *   - sm_90a (H100) only; there is no CPU fallback
  */
 #ifndef NEURAY_B200_H
 #define NEURAY_B200_H
@@ -421,8 +421,8 @@ int nr_consistency_loss(const float* prob0, const float* prob1, int qn, int rn, 
 
 /* ---- diagnostics ------------------------------------------------------------------------------------------- */
 
-/* Self-test of the tcgen05 layer primitive the point kernel uses: D[128,n] = A[128,k] * W[n,k]^T with A staged in
- * TMEM and W in swizzled shared memory; mode 0 = one TF32 pass, 1 = 3xTF32 (fp32-accurate).  (n,k) in
+/* Self-test of the wgmma layer primitive the point kernel uses: D[128,n] = A[128,k] * W[n,k]^T with A in the shared-memory
+ * activation tile and W in swizzled shared memory; mode 0 = one TF32 pass, 1 = 3xTF32 (fp32-accurate).  (n,k) in
  * {(32,32),(64,64),(16,64)}. */
 int nr_tc_selftest(const float* A, const float* W, float* D, int n, int k, int mode, void* stream);
 

@@ -1,4 +1,4 @@
-"""neuray_b200 -- B200-native (sm_100a) implementation of NeuRay's per-ray rendering hot path.
+"""neuray_b200 -- H100-native (sm_90a) implementation of NeuRay's per-ray rendering hot path.
 
 Drop-in surface (SURVEY.md section 8b):
     neuray_b200.render_ops      mirrors reference network/render_ops.py (same 12 function names)

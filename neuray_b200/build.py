@@ -1,4 +1,4 @@
-"""In-tree build of libneuray_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+"""In-tree build of libneuray_b200.so for sm_90a (nvcc cross-compiles without a GPU).
 
     python -m neuray_b200.build [--force] [--verbose]
 
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libneuray_b200.so")
 SOURCES = ["nr_ops.cu", "nr_pack.cu", "nr_point_kernel.cu", "nr_ray_kernel.cu", "nr_tc_test.cu", "nr_train.cu", "nr_tape_gemm.cu", "nr_encoder.cu", "nr_losses.cu", "nr_mvs.cu"]
 HEADERS = ["nr_common.cuh", "nr_resample.cuh", "nr_tc.cuh", "nr_point_kernel_pm3.cuh", "nr_train_math.cuh", "nr_conv.cuh", "nr_loss_math.cuh", "nr_mvs.cuh", "nr_mvs_graph.cuh", "nr_encoder_graph.cuh", os.path.join("..", "..", "include", "neuray_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 
 
@@ -45,7 +45,7 @@ def build(force=False, verbose=False):
             print(out)
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -116,7 +116,7 @@ static_assert(GRP_B % 4 == 0 && HOIST_W % 4 == 0 && BASE0_W % 4 == 0 && BASE1_W 
 }  // namespace lay
 
 // ------------------------------------------------------------------------------------------------------------
-// Tensor-core weight buffer (w_tc): every tcgen05 layer's W^T as hi / lo tf32 parts, K padded and re-ordered to the
+// Tensor-core weight buffer (w_tc): every tensor-core layer's W^T as hi / lo tf32 parts, K padded and re-ordered to the
 // kernel's A-column order, pre-swizzled into K-major SWIZZLE_128B tiles of 32-wide K slabs, grouped into the 16 KB
 // ring stages the producer warp streams (offsets in floats).  Inside a stage:
 //   head h   : L0 hi 0 | L0 lo 1024 | L1 hi 2048 | L1 lo 3072                     (N 32, K 32)
@@ -151,7 +151,7 @@ constexpr int TOTAL = G0 + 3 * STAGE;
 //   * exp through ex2.approx.ftz (FMUL + MUFU; __expf's non-ftz path adds a compare and two predicated multiplies per
 //     call for denormal results, which only matter below exp(-87) where ELU is -1 either way); abs error ~1e-7
 //   * the select is a selp on a setp, never a divergent branch around the MUFU (the ternary form compiled to one and
-//     serialised the 32-wide epilogues; profiles/r1_phase_timing.md)
+//     serialised the 32-wide epilogues)
 __device__ __forceinline__ float ex2_ftz(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

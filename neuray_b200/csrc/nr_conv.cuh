@@ -28,7 +28,7 @@ namespace cv {
 
 constexpr int THREADS = 256;   // 8 warps: WM = 8 / WN along M x WN = Cout / 32 along N; a warp owns 16*MT pixels x 32 channels
 // Output pixels per CTA: BM in {64, 128, 256}, MT = BM / (16 WM) m16 tiles per warp.  128 is the default; 64 for Cout = 128 when
-// 128-pixel tiles would leave a nearly empty last wave (layer3 of an 800x800 frame: 157 tiles on 148 SMs); 256 for Cout = 32,
+// 128-pixel tiles would leave a nearly empty last wave (layer3 of an 800x800 frame: 157 tiles on 132 SMs); 256 for Cout = 32,
 // where a warp otherwise owns a single m16 tile and re-reads / re-splits the whole weight tile for 12 MMAs (2 pipeline stages
 // instead of 3, so that two CTAs still fit an SM).
 __host__ __device__ constexpr int mt_of(int BM, int BN) { return BM / (16 * (8 / (BN / 32))); }

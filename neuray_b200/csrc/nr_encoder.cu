@@ -144,7 +144,7 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
 
   // InstanceNorm sums: thread partials -> the 8 row lanes of a warp (shuffles) -> the CTA (shared memory) -> ONE fp64 atomic
   // per (column, sum) and CTA.  Thousands of CTAs adding to the same 2 x Cout addresses of an image serialise in L2: with one
-  // atomic per warp the 2 500-CTA layers spent 300 us of their 420 us on them (profiles/r2_encoders_v0_launches.md).
+  // atomic per warp the large-CTA-count layers spent most of their time on them.
   __shared__ double cta_sums[2 * 128];
   const long long M = (long long)p.N * p.Ho * p.Wo;
   const long long plane = (long long)p.Ho * p.Wo;
@@ -486,7 +486,7 @@ int sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 148;
+  return sms > 0 ? sms : 132;
 }
 
 int pack_params(const enc::NetSpec& spec, const float* const* params, int n_params, float* packed, cudaStream_t st) {

@@ -178,7 +178,7 @@ extern "C" int nr_mvsnet_fwd(const float* packed, const NrMvsIn* a, float* prob,
   mvs::MvsNet net;
   mvs::build_mvsnet(net);
   enc::Arena ar{(char*)workspace, size_t(workspace_bytes), 0, true};
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   mvs::StreamOps ops{(cudaStream_t)stream, sms, NR_OK};

@@ -58,7 +58,7 @@ NR_HD void axpy_row(float xv, const float* __restrict__ wr, float (&acc)[COUT]) 
 
 // One thread = one output voxel x one group of COUT consecutive output channels (group g of p.Cout / COUT): the layers with 32 / 64
 // outputs sit on 25 600 / 3 200 voxels, far too few threads for the machine if a thread carried all of a voxel's outputs
-// (profiles/r2_cost_volume_launches.md: 750 us for 110 592 serial FMAs per thread on 25 CTAs).
+// (a thread carrying all outputs of a voxel ran ~110 000 serial FMAs on a few dozen CTAs).
 template <int COUT>
 NR_HD void conv_voxel(const ConvP& p, long long v, int g, float (&acc)[COUT]) {
   const int wo = int(v % p.Wo);

@@ -303,8 +303,8 @@ int nr_pack_feature_maps(const float* ray_feats, const float* img_feats, const f
   NR_CHECK_ARG(rfn >= 1 && rfn <= NR_MAX_VIEWS && h > 1 && w > 1 && fh > 0 && fw > 0, "shape");
   cudaStream_t s = (cudaStream_t)stream;
   const long long nf = (long long)rfn * fh * fw * 16, nr_ = (long long)rfn * h * w;
-  if (maps) pack_feat_kernel<<<min(blocks_for(nf), 148 * 16), TPB, 0, s>>>(ray_feats, img_feats, rfn, fh, fw, out_feat);
-  pack_rgb_kernel<<<min(blocks_for(nr_), 148 * 16), TPB, 0, s>>>(imgs, rfn, h, w, out_rgb);
+  if (maps) pack_feat_kernel<<<min(blocks_for(nf), 132 * 16), TPB, 0, s>>>(ray_feats, img_feats, rfn, fh, fw, out_feat);
+  pack_rgb_kernel<<<min(blocks_for(nr_), 132 * 16), TPB, 0, s>>>(imgs, rfn, h, w, out_rgb);
   NR_CHECK_LAUNCH("pack_feature_maps");
   return NR_OK;
 }
@@ -379,7 +379,7 @@ int nr_project_points(const float* pts, int pn, const float* view_params, int rf
                       float* depth, float* mask, float* valid_z, void* stream) {
   if (pn == 0) return NR_OK;   // empty input: nothing to do (pointers of empty tensors are null)
   NR_CHECK_ARG(pts && view_params && pn >= 0 && rfn >= 1, "project_points arguments");
-  project_kernel<<<min(blocks_for((long long)pn * rfn), 148 * 32), TPB, 0, (cudaStream_t)stream>>>(pts, pn, view_params, rfn, h, w,
+  project_kernel<<<min(blocks_for((long long)pn * rfn), 132 * 32), TPB, 0, (cudaStream_t)stream>>>(pts, pn, view_params, rfn, h, w,
                                                                                                   dir, pix, depth, mask, valid_z);
   NR_CHECK_LAUNCH("project_points");
   return NR_OK;
@@ -389,7 +389,7 @@ int nr_interpolate_feats(const float* feats, const float* pts, const float* mask
                          float w, int border, int align_corners, float* out, void* stream) {
   if (n == 0) return NR_OK;   // empty input: nothing to do (pointers of empty tensors are null)
   NR_CHECK_ARG(feats && pts && out && b >= 1 && c >= 1 && fh >= 1 && fw >= 1 && n >= 0, "interpolate_feats arguments");
-  interp_kernel<<<min(blocks_for((long long)b * n), 148 * 32), TPB, 0, (cudaStream_t)stream>>>(feats, pts, mask, b, c, fh, fw, n, h, w,
+  interp_kernel<<<min(blocks_for((long long)b * n), 132 * 32), TPB, 0, (cudaStream_t)stream>>>(feats, pts, mask, b, c, fh, fw, n, h, w,
                                                                                               border, align_corners, out);
   NR_CHECK_LAUNCH("interpolate_feats");
   return NR_OK;
@@ -399,7 +399,7 @@ int nr_interpolate_feats_bwd(const float* d_out, const float* pts, const float* 
                              float w, int border, int align_corners, float* d_feats, void* stream) {
   if (n == 0) return NR_OK;
   NR_CHECK_ARG(d_out && pts && d_feats && b >= 1 && c >= 1 && fh >= 1 && fw >= 1 && n >= 0, "interpolate_feats_bwd arguments");
-  interp_bwd_kernel<<<min(blocks_for((long long)b * n), 148 * 32), TPB, 0, (cudaStream_t)stream>>>(d_out, pts, mask, b, c, fh, fw, n, h,
+  interp_bwd_kernel<<<min(blocks_for((long long)b * n), 132 * 32), TPB, 0, (cudaStream_t)stream>>>(d_out, pts, mask, b, c, fh, fw, n, h,
                                                                                                   w, border, align_corners, d_feats);
   NR_CHECK_LAUNCH("interpolate_feats_bwd");
   return NR_OK;
@@ -419,7 +419,7 @@ int nr_sample_fine_depth(const float* depth, const float* hit_prob, const float*
   NR_CHECK_ARG(smem <= 200 * 1024, "sample_fine_depth shared memory");
   if (smem > 48 * 1024)   // per-device attribute, set per launch: no per-process state (see nr_point_kernel.cu)
     cudaFuncSetAttribute(fine_depth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-  const int grid = min((rn + warps - 1) / warps, 148 * 8);
+  const int grid = min((rn + warps - 1) / warps, 132 * 8);
   fine_depth_kernel<<<grid, warps * 32, smem, (cudaStream_t)stream>>>(depth, hit_prob, depth_range, rn, dn, fine_dn, u, u_stride,
                                                                       use_all, do_sort, sort_n, per_warp, out);
   NR_CHECK_LAUNCH("sample_fine_depth");
@@ -533,7 +533,7 @@ extern "C" int nr_diff_feats(const float* imgs, const float* depth_in, const flo
   NR_CHECK_ARG(imgs && depth_in && poses && Ks && view_params && out, "null device pointer");
   NR_CHECK_ARG(rfn >= 1 && rfn <= NR_MAX_VIEWS && h > 1 && w > 1, "shape");
   const long long total = (long long)rfn * h * w;
-  ops::diff_feats_kernel<<<min(ops::blocks_for(total), 148 * 16), ops::TPB, 0, (cudaStream_t)stream>>>(imgs, depth_in, poses, Ks, view_params,
+  ops::diff_feats_kernel<<<min(ops::blocks_for(total), 132 * 16), ops::TPB, 0, (cudaStream_t)stream>>>(imgs, depth_in, poses, Ks, view_params,
                                                                                                     rfn, h, w, out);
   NR_CHECK_LAUNCH("diff_feats");
   return NR_OK;

@@ -1,14 +1,15 @@
 // Point kernel (namespace nr::pkt): everything of a render pass that is per (point, view) row, the cross-view pooling and
 // the per-point layers -- reference renderer.py:171-178 up to geometry_fc, ibrnet.py:315-354.  One kernel
-// (nr_point_kernel_pm3.cuh, three 128-row blocks per SM); this file holds what its pieces share and the launcher:
+// (nr_point_kernel_pm3.cuh, one 128-row block per SM); this file holds what its pieces share and the launcher:
 //
-//   * thread r owns (point,view) row r of a 128-row block = TMEM lane r (a warp may only touch its own 32-lane TMEM
-//     quadrant, which is exactly "its" rows); row = point * G + view, G = lanes per point = power of two >= rfn
-//   * a layer  D[128 x N] += A[128 x K] * W^T :  A (hi and lo parts of the 3xTF32 split) is written to TMEM by the row
-//     owners with tcgen05.st, W^T (hi / lo, pre-split and pre-swizzled by nr_pack_weights) sits in shared memory, D comes
-//     back with tcgen05.ld for the bias / activation epilogue, whose result goes straight back to TMEM as the next A
-//   * weights stream through a 3 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk); full/empty
-//     mbarriers, the "empty" arrivals are tcgen05.commit of the consuming MMAs
+//   * thread r of the block's warp group owns (point,view) row r of the 128-row block = row r of its shared-memory
+//     activation tile; row = point * G + view, G = lanes per point
+//   * a layer  D[128 x N] += A[128 x K] * W^T :  A (hi and lo parts of the 3xTF32 split) is written into the activation
+//     tile by the row owners, W^T (hi / lo, pre-split and pre-swizzled by nr_pack_weights) sits in shared memory, the warp
+//     group multiplies them with wgmma and writes D back into the tile for the bias / activation epilogue, whose result
+//     goes back into the tile as the next A
+//   * weights stream through a 4 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk); full/empty
+//     mbarriers, the "empty" arrival comes from the block once the consuming wgmma have completed
 #include <type_traits>
 
 #include "nr_common.cuh"
@@ -21,11 +22,7 @@ __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpre
 
 constexpr int REC = NR_POINT_REC;
 constexpr int RING_STAGE = 4096;    // 16 KB
-constexpr int NBUF = 4;             // depth of the shared weight ring.  The three blocks of a CTA consume every stage, so the depth bounds how far
-                                    // they can drift apart: 3 -> 4 slots = +1.9 % (166.6 -> 169.8 M); more does not fit next to the resident
-                                    // base_fc.0 tile, and streaming that tile too (19 stages per tile, 6..9 slots) costs 13..18 %.
-                                    // Also measured and rejected (profiles/README.md): feeding from all three blocks through a shared
-                                    // claim counter (-9 %), feeding from a non-issuing warp of block 0 (-2.5 %), a non-inlined feed (-12 %)
+constexpr int NBUF = 4;             // depth of the shared weight ring (the three base_fc.0 stages are held at once, so at least 3)
 constexpr int SW = 2048;
 
 // ---- small resident weights (floats inside `sw`) ----
@@ -44,32 +41,39 @@ struct KParams {
   int P, n_tiles, n_heads;
 };
 
+// One ring stage from w_tc: up to two bulk copies (source offset in floats, bytes) x2, the second landing right behind the first
+__device__ __forceinline__ void load_stage(float* slot, const float* w_tc, int4 e, uint64_t* full) {
+  tc::mbar_arrive_expect_tx(full, uint32_t(e.y + e.w));
+  tc::bulk_g2s(slot, w_tc + e.x, e.y, full);
+  if (e.w) tc::bulk_g2s(slot + e.y / 4, w_tc + e.z, e.w, full);
+}
+
 // The weight stream, driven by ONE thread (thread 0) from inside its own MMA-issue path: before it waits for a stage it
 // issues every stage up to that one (blocking on the ring slot if it has to) and opportunistically up to NBUF-1 further.
 struct Producer {
   const float* w_tc;
   float* ring;
   uint64_t *wfull, *wempty;
-  const int2* table;      // shared: per stage of a tile (source offset in floats, bytes), built once at kernel start
+  const int4* table;      // shared: per stage of a tile (load_stage's copies), built once at kernel start
   uint32_t next;          // next stage index to issue
   uint32_t total;         // iters * stages_per_tile
   int stages_per_tile;
   int s;                  // next % stages_per_tile, kept as a running counter (this code runs on one lane, inside block 0's MMA-issue
                           // path: every instruction counts)
 
-  // (source offset, bytes) of stage s of a tile: heads, prob_embed x2, base_fc.0 x3, base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
-  __device__ static int2 stage_source(int s, int n_heads) {
-    if (s < n_heads) return make_int2(tcl::HEAD0 + s * RING_STAGE, RING_STAGE * 4);
+  // copies of stage s of a tile: heads, prob_embed x2, base_fc.0 x3, the view-pooled base_fc.0 inputs x5 (hi slab | lo slab
+  // of the resident-layout HST tile), base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
+  __device__ static int4 stage_source(int s, int n_heads) {
+    if (s < n_heads) return make_int4(tcl::HEAD0 + s * RING_STAGE, RING_STAGE * 4, 0, 0);
     const int t = s - n_heads;
-    const int src = t == 0 ? tcl::PE0 : t == 1 ? tcl::PE1 : t <= 4 ? tcl::B0 + (t - 2) * RING_STAGE : t == 5 ? tcl::B1 : t == 6 ? tcl::V01
-                  : t == 7 ? tcl::V2R : tcl::G0 + (t - 8) * RING_STAGE;
-    return make_int2(src, t == 1 ? 3072 * 4 : RING_STAGE * 4);
+    if (t >= 5 && t < 10) return make_int4(tcl::HST + (t - 5) * 2048, 2048 * 4, tcl::HST + tcl::HST_SIZE / 2 + (t - 5) * 2048, 2048 * 4);
+    const int src = t == 0 ? tcl::PE0 : t == 1 ? tcl::PE1 : t <= 4 ? tcl::B0 + (t - 2) * RING_STAGE : t == 10 ? tcl::B1 : t == 11 ? tcl::V01
+                  : t == 12 ? tcl::V2R : tcl::G0 + (t - 13) * RING_STAGE;
+    return make_int4(src, t == 1 ? 3072 * 4 : RING_STAGE * 4, 0, 0);
   }
   __device__ __forceinline__ void issue() {
-    const int2 e = table[s];
     const uint32_t buf = next % NBUF;
-    tc::mbar_arrive_expect_tx(wfull + buf, e.y);
-    tc::bulk_g2s(ring + buf * RING_STAGE, w_tc + e.x, e.y, wfull + buf);
+    load_stage(ring + buf * RING_STAGE, w_tc, table[s], wfull + buf);
     ++next;
     if (++s == stages_per_tile) s = 0;
   }
@@ -88,16 +92,14 @@ struct Producer {
 
 // Everything a compute thread needs to drive its block's tensor-core layers.
 struct Blk {
-  uint32_t tAhi, tAlo, tD;      // TMEM addresses of this thread's lane quadrant (lane field included)
-  uint32_t mAhi, mAlo, mD;      // same columns, lane 0: what the MMA instruction takes
-  uint64_t* mma_bar;
+  float* act;                   // the block's activation tile (tc::act_index)
+  uint32_t act_addr;            // its shared-space byte address
+  int row;                      // this thread's row of the tile = its index in the warp group
   uint64_t *wfull, *wempty;     // arrays [NBUF]
   uint32_t ring_addr;           // shared-space byte address of the ring
-  uint32_t phase;               // parity of the next mma_bar completion
   uint32_t wi;                  // weight stages consumed so far (same sequence in every thread)
   int blk;
   bool leader;
-  bool issuer_warp;             // warp 0 of the block (warp-uniform): one elected lane of it issues the MMAs
   Producer* prod;               // non-null in the one thread that also feeds the weight ring (point-major kernel)
   long long* tk;                // diagnostics: where run_layer drops clock64() stamps (nullptr: off)
 };

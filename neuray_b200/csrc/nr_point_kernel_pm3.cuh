@@ -1,21 +1,22 @@
-// Point kernel (namespace nr::pkt::pm3): point-major rows, tcgen05 layers, THREE independent 128-row blocks per SM.
+// Point kernel (namespace nr::pkt::pm3): point-major rows, wgmma layers, one 128-row block per SM.
 //
-// Row = point * G + view inside a block (G lanes per point: 4, 5, 6, 8, 10, 16 or 32), thread r = row r = TMEM lane r; a thread
-// keeps its row in registers from the gather to the output record.  Resource plan (one CTA per SM: 384 compute threads + a
-// 128-thread producer group whose lane 0 feeds the weight ring, see NR_PRODUCER_WARP below):
-//   * tensor memory: 160 columns per block.  Activations: hi parts at columns [0,64), lo parts at [64,128), accumulator at
-//     [128,160).  base_fc.0 (N = 64) is issued in K rounds into one accumulator at [96,160): round A (the 32 neuray_feat
-//     inputs) right after prob_embed.2 while they are still the only live A operand, round B (the 40 rgb_feat inputs, lo parts
-//     at [48,88)) after ray_dir_fc, then five rounds of view-pooled statistics (K 32 each).  Its epilogue reads the accumulator
-//     half by half and writes base_fc.2's operand over the columns it has already consumed.
-//   * shared memory (230 KB): 4 x 16 KB weight ring (TMA bulk copies, fed by the producer group), the resident tiles of the pooled
-//     base_fc.0 inputs (80 KB) and of ray_dir_fc.2, small weights, camera blocks, and one [32][36] transposition buffer per warp:
-//     gather (two channel passes: ray_feats, then img_feats, which stay there until ray_dir_fc needs them), the cross-view
-//     pooling (pm::pool_rows) and the lane-group sums of the non-power-of-two groups all go through it.
-//   * 384 compute threads: three warps per SM sub-partition; the CTA launches at 512 x 128 registers and setmaxnreg moves the
-//     producer group's share to the compute groups (160 / 24 registers per thread).
-// The three blocks exist to fill each other's bubbles: a block has ~25 MMA round trips per tile during which its four warps
-// have nothing to do (profiles/r2_point_kernel_v4_lines.txt).
+// Row = point * G + view inside a block (G lanes per point: 4, 5, 6, 8, 10, 16 or 32), thread r of the block's warp group =
+// row r of the activation tile; a thread keeps its row in registers from the gather to the output record.  Resource plan
+// (one CTA per SM: 128 compute threads + a 128-thread producer group whose lane 0 feeds the weight ring, see
+// NR_PRODUCER_WARP below):
+//   * activation tile (80 KB of shared memory, 160 columns x 128 rows, tc::act_index): hi parts at columns [0,64), lo parts
+//     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) is issued in K rounds into one accumulator at [96,160):
+//     round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only live A operand, round B
+//     (the 40 rgb_feat inputs, lo parts at [48,88)) after ray_dir_fc, then five rounds of view-pooled statistics (K 32
+//     each).  Its epilogue reads the accumulator half by half and writes base_fc.2's operand over the columns it has
+//     already consumed.
+//   * the rest of shared memory: 4 x 16 KB weight ring (TMA bulk copies, fed by the producer group; the view-pooled
+//     base_fc.0 inputs stream through it as five more stages), the resident tile of ray_dir_fc.2, small weights, camera
+//     blocks, and one [32][36] transposition buffer per warp: gather (two channel passes: ray_feats, then img_feats, which
+//     stay there until ray_dir_fc needs them), the cross-view pooling (pm::pool_rows) and the lane-group sums of the
+//     non-power-of-two groups all go through it.
+//   * a layer is one wgmma round trip of the warp group (issue, wait, accumulator back into the tile): the 227 KB of shared
+//     memory hold one activation tile next to the ring, so a second block per SM would have to give up the ring.
 #pragma once
 
 namespace pm3 {
@@ -32,27 +33,26 @@ using pm::gmax_np2;
 using pm::gsum4_np2;
 
 #ifndef NR_GATHER_BATCH
-#define NR_GATHER_BATCH 2     // 4 (16 loads in flight per lane) cost 520 B of spills per thread and 12 % of the kernel (profiles/README.md)
+#define NR_GATHER_BATCH 2     // 4 (16 loads in flight per lane) spills
 #endif
 constexpr int GB = NR_GATHER_BATCH;                           // rows whose 4 taps a quarter-warp keeps in flight at once (4 x GB 128-bit loads per lane)
 #ifndef NR_GATHER_OVERLAP
 #define NR_GATHER_OVERLAP 1
 #endif
-constexpr int NBLK = 3;
+constexpr int NBLK = 1;
 #ifndef NR_PRODUCER_WARP
 #define NR_PRODUCER_WARP 1
 #endif
 constexpr int NCOMP = NBLK * 128;
-// + one warp group whose lane 0 does nothing but keep the weight ring full.  Registers are handed out per 4 warps, so the
-// CTA launches at 512 x 128 and the producer group gives its registers to the compute groups (setmaxnreg below).
+// + one warp group whose lane 0 does nothing but keep the weight ring full
 constexpr int NTHR = NCOMP + (NR_PRODUCER_WARP ? 128 : 0);
-constexpr int REGS_COMPUTE = 160, REGS_PRODUCER = 24;
-constexpr int TCOLS = 160;                                    // tensor-memory columns per block
+constexpr int TCOLS = 160;                                    // activation-tile columns per block
+constexpr int ACT = (TCOLS / 32) * 4096;                      // floats per activation tile
 
 // ---- shared memory map (floats) ----
 constexpr int OFF_RING = 0;                                   // NBUF x RING_STAGE
-constexpr int OFF_HST = OFF_RING + NBUF * RING_STAGE;         // view-pooled part of base_fc.0, tensor-core tile (resident, 1024-byte aligned)
-constexpr int OFF_RD1 = OFF_HST + tcl::HST_SIZE;              // ray_dir_fc.2 tensor-core tile (resident, 1024-byte aligned)
+constexpr int OFF_ACT = OFF_RING + NBUF * RING_STAGE;         // NBLK activation tiles (1024-byte aligned)
+constexpr int OFF_RD1 = OFF_ACT + NBLK * ACT;                 // ray_dir_fc.2 tensor-core tile (resident, 1024-byte aligned)
 constexpr int OFF_WG1 = OFF_RD1 + tcl::RD1_SIZE;              // geometry_fc.2: [16][64] (output-major, columns in own_col order) | bias[16]
 constexpr int WG1 = 64 * 16 + 16;
 constexpr int OFF_SW = OFF_WG1 + WG1;                         // small resident weights (offsets SW_*, nr_point_kernel.cu)
@@ -61,138 +61,143 @@ constexpr int STG_ROW = 36;
 constexpr int STG = (NCOMP / 32) * 32 * STG_ROW;
 constexpr int OFF_CAM = OFF_STG + STG;                        // que_cam [24] (padded to 32) | view_params [NR_MAX_VIEWS][20]
 constexpr int CAM = 32 + NR_MAX_VIEWS * 20;
-constexpr int OFF_STAB = OFF_CAM + CAM;                       // Producer::table: int2 per stage of a tile (at most 4 + 11)
-constexpr int OFF_BAR = OFF_STAB + 32;
+constexpr int OFF_STAB = OFF_CAM + CAM;                       // Producer::table: int4 per stage of a tile (at most 4 + 16)
+constexpr int OFF_BAR = OFF_STAB + 80;
 constexpr int SMEM_FLOATS = OFF_BAR + 32;
 constexpr size_t SMEM_BYTES = size_t(SMEM_FLOATS) * 4;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-static_assert((OFF_HST * 4) % 1024 == 0 && (OFF_RD1 * 4) % 1024 == 0 && OFF_WG1 % 4 == 0 && OFF_SW % 4 == 0 && OFF_STG % 4 == 0, "alignment");
+static_assert(OFF_STAB % 4 == 0, "alignment");
+static_assert((OFF_ACT * 4) % 1024 == 0 && (OFF_RD1 * 4) % 1024 == 0 && OFF_WG1 % 4 == 0 && OFF_SW % 4 == 0 && OFF_STG % 4 == 0, "alignment");
 
-// Layer issue, executed by all 128 threads of the block after they wrote their A columns (b.tAhi / b.mAhi = column 0 of
-// the block).  K chunk c (of NCH) reads A columns AHI + 8c (c < NLIN) or TAILHI + 8(c - NLIN), lo parts LOOFF columns
-// further, and B chunk CB0 + c of the layer's tiles (slab (CB0+c)/4; one ring stage per slab when NSTG > 1); ACC: the
-// first MMA accumulates onto what is already in D.
+// Layer issue, executed by all 128 threads of the block after they wrote their A columns.  K chunk c (of NCH) reads A
+// columns AHI + 8c (c < NLIN) or TAILHI + 8(c - NLIN), lo parts LOOFF columns further, and B chunk CB0 + c of the layer's
+// tiles (slab (CB0+c)/4; one ring stage per slab when NSTG > 1); ACC: the first MMA accumulates onto what is already in the
+// accumulator columns [DCOL, DCOL + N).  Returns with the outputs in the activation tile, visible to every row owner.
 template <int N, int NCH, int AHI, int LOOFF, int NLIN, int TAILHI, int DCOL, int CB0, int NSTG, uint32_t OFF_HI, uint32_t OFF_LO,
           uint32_t SLAB, bool WAIT_FULL, bool RELEASE, bool ACC>
 __device__ __forceinline__ void issue_layer(Blk& b) {
   // b.tk: diagnostics of ONE layer's round trip (debug instantiation only; a compile-time null otherwise)
   if (b.tk) b.tk[0] = clock64();
-  tc::tmem_st_wait();
-  tc::fence_before_thread_sync();
+  tc::fence_proxy_async_smem();              // this thread's A columns -> visible to the tensor cores
   if (b.tk) b.tk[1] = clock64();
   tc::named_sync(2 + b.blk, 128);
   if (b.tk) b.tk[2] = clock64();
-  if (b.issuer_warp) {                       // warp-uniform branch; one elected lane issues
-    tc::fence_after_thread_sync();
-    const uint32_t st0 = b.wi % NBUF;
-    if (WAIT_FULL && b.prod != nullptr) b.prod->feed(b.wi + NSTG - 1);
-    __syncwarp();
-    if (WAIT_FULL) {
+  const uint32_t st0 = b.wi % NBUF;
+  if (WAIT_FULL && b.prod != nullptr) b.prod->feed(b.wi + NSTG - 1);
+  if (WAIT_FULL) {
 #pragma unroll
-      for (int s = 0; s < NSTG; ++s) tc::mbar_wait(b.wfull + ((st0 + s) % NBUF), ((b.wi + s) / NBUF) & 1);
-    }
-    if (b.tk) b.tk[3] = clock64();
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::idesc_tf32(N);
-      uint64_t dhi[NSTG], dlo[NSTG];
-#pragma unroll
-      for (int s = 0; s < NSTG; ++s) {
-        const uint32_t base = b.ring_addr + ((st0 + s) % NBUF) * (RING_STAGE * 4);
-        dhi[s] = tc::smem_desc_sw128(base + OFF_HI);
-        dlo[s] = tc::smem_desc_sw128(base + OFF_LO);
-      }
-#pragma unroll
-      for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          const int acol = (c < NLIN ? AHI + 8 * c : TAILHI + 8 * (c - NLIN)) + (ps == 1 ? LOOFF : 0);
-          const int cb = CB0 + c;
-          const int slab = cb >> 2;
-          const int stg = NSTG == 1 ? 0 : slab;
-          const uint32_t inc = ((NSTG == 1 ? slab * SLAB : 0u) + (cb & 3) * 32) >> 4;
-          tc::mma_tf32_ts(b.mAhi + DCOL, b.mAhi + acol, (ps == 2 ? dlo[stg] : dhi[stg]) + inc, idesc, ACC || (ps | c) != 0);
-        }
-      }
-      if (RELEASE) {
-#pragma unroll
-        for (int s = 0; s < NSTG; ++s) tc::mma_commit(b.wempty + ((st0 + s) % NBUF));
-      }
-      tc::mma_commit(b.mma_bar);
-    }
-    __syncwarp();
-    if (b.tk) b.tk[4] = clock64();
+    for (int s = 0; s < NSTG; ++s) tc::mbar_wait(b.wfull + ((st0 + s) % NBUF), ((b.wi + s) / NBUF) & 1);
   }
-  if (RELEASE) b.wi += NSTG;
+  if (b.tk) b.tk[3] = clock64();
+  float d[2][N / 2];
+  if (ACC) tc::acc_load<N>(b.act, DCOL, b.row, d);
+  else {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
+  }
+  uint64_t dhi[NSTG], dlo[NSTG];
+#pragma unroll
+  for (int s = 0; s < NSTG; ++s) {
+    const uint32_t base = b.ring_addr + ((st0 + s) % NBUF) * (RING_STAGE * 4);
+    dhi[s] = tc::smem_desc_sw128(base + OFF_HI);
+    dlo[s] = tc::smem_desc_sw128(base + OFF_LO);
+  }
+  tc::wgmma_fence();
+#pragma unroll
+  for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const int acol = (c < NLIN ? AHI + 8 * c : TAILHI + 8 * (c - NLIN)) + (ps == 1 ? LOOFF : 0);
+      const int cb = CB0 + c;
+      const int slab = cb >> 2;
+      const int stg = NSTG == 1 ? 0 : slab;
+      const uint32_t inc = ((NSTG == 1 ? slab * SLAB : 0u) + (cb & 3) * 32) >> 4;
+      const uint64_t bd = (ps == 2 ? dlo[stg] : dhi[stg]) + inc;
+      tc::wgmma_tf32<N>(d[0], tc::act_desc(b.act_addr, acol, 0), bd);
+      tc::wgmma_tf32<N>(d[1], tc::act_desc(b.act_addr, acol, 1), bd);
+    }
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait_all();
+  if (b.tk) b.tk[4] = clock64();
+  tc::acc_store<N>(b.act, DCOL, b.row, d);
+  tc::named_sync(2 + b.blk, 128);            // outputs in the tile; every warp's reads of the stages have completed
+  if (RELEASE) {
+    if (b.leader) {
+#pragma unroll
+      for (int s = 0; s < NSTG; ++s) tc::mbar_arrive(b.wempty + ((st0 + s) % NBUF));
+    }
+    b.wi += NSTG;
+  }
+  if (b.tk) b.tk[5] = clock64();
 }
 // Same, B operand = a resident shared-memory tile at byte address `base` (hi slabs first, SLAB bytes apart; lo parts
-// OFF_LO bytes further): no ring accounting.  `issuer`: warp-uniform, true in the one warp of the block that issues
-// this layer (a completion wait separates consecutive layers, so different layers may be issued by different warps).
+// OFF_LO bytes further): no ring accounting.
 template <int N, int NCH, int AHI, int LOOFF, int DCOL, int CB0, uint32_t OFF_LO, uint32_t SLAB, bool ACC>
-__device__ __forceinline__ void issue_layer_resident(Blk& b, uint32_t base, bool issuer) {
-  tc::tmem_st_wait();
-  tc::fence_before_thread_sync();
+__device__ __forceinline__ void issue_layer_resident(Blk& b, uint32_t base) {
+  tc::fence_proxy_async_smem();
   tc::named_sync(2 + b.blk, 128);
-  if (issuer) {
-    tc::fence_after_thread_sync();
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::idesc_tf32(N);
-      const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + OFF_LO);
+  float d[2][N / 2];
+  if (ACC) tc::acc_load<N>(b.act, DCOL, b.row, d);
+  else {
 #pragma unroll
-      for (int ps = 0; ps < 3; ++ps) {
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-          const int acol = AHI + 8 * c + (ps == 1 ? LOOFF : 0);
-          const int cb = CB0 + c;
-          const uint32_t inc = ((cb >> 2) * SLAB + (cb & 3) * 32) >> 4;
-          tc::mma_tf32_ts(b.mAhi + DCOL, b.mAhi + acol, (ps == 2 ? dlo : dhi) + inc, idesc, ACC || (ps | c) != 0);
-        }
-      }
-      tc::mma_commit(b.mma_bar);
-    }
-    __syncwarp();
+      for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
   }
-}
-__device__ __forceinline__ void wait_layer(Blk& b) {
-  tc::mbar_wait(b.mma_bar, b.phase);
-  b.phase ^= 1;
-  tc::fence_after_thread_sync();
-  if (b.tk) b.tk[5] = clock64();
+  const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + OFF_LO);
+  tc::wgmma_fence();
+#pragma unroll
+  for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const int acol = AHI + 8 * c + (ps == 1 ? LOOFF : 0);
+      const int cb = CB0 + c;
+      const uint32_t inc = ((cb >> 2) * SLAB + (cb & 3) * 32) >> 4;
+      const uint64_t bd = (ps == 2 ? dlo : dhi) + inc;
+      tc::wgmma_tf32<N>(d[0], tc::act_desc(b.act_addr, acol, 0), bd);
+      tc::wgmma_tf32<N>(d[1], tc::act_desc(b.act_addr, acol, 1), bd);
+    }
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait_all();
+  tc::acc_store<N>(b.act, DCOL, b.row, d);
+  tc::named_sync(2 + b.blk, 128);
 }
 // the common case: activations hi [0,64) / lo [64,128), accumulator at 128, one ring stage
 template <int N, int NCH, int AHI, int NLIN, int TAILHI, uint32_t OFF_HI, uint32_t OFF_LO, uint32_t SLAB, bool WAIT_FULL, bool RELEASE>
 __device__ __forceinline__ void run_layer(Blk& b) {
   issue_layer<N, NCH, AHI, 64, NLIN, TAILHI, 128, 0, 1, OFF_HI, OFF_LO, SLAB, WAIT_FULL, RELEASE, false>(b);
-  wait_layer(b);
 }
 
-__device__ __forceinline__ void ld32(const Blk& b, int col, float* v) {
-  tc::tmem_ld16(b.tAhi + col, v);
-  tc::tmem_ld16(b.tAhi + col + 16, v + 16);
-  tc::tmem_ld_wait();
+// this thread's row of the activation tile: columns [col, col + 4Q), col a multiple of 4
+template <int Q>
+__device__ __forceinline__ void ld_row(const Blk& b, int col, float* v) {
+#pragma unroll
+  for (int q = 0; q < Q; ++q) {
+    const float4 t = *reinterpret_cast<const float4*>(b.act + tc::act_index(b.row, col + 4 * q));
+    v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+  }
 }
-__device__ __forceinline__ void ld16(const Blk& b, int col, float* v) {
-  tc::tmem_ld16(b.tAhi + col, v);
-  tc::tmem_ld_wait();
+template <int Q>
+__device__ __forceinline__ void st_split(const Blk& b, int hi, int lo, const float* v) {
+#pragma unroll
+  for (int q = 0; q < Q; ++q) {
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tc::split_tf32(v[4 * q + j], h[j], l[j]);
+    *reinterpret_cast<uint4*>(b.act + tc::act_index(b.row, hi + 4 * q)) = make_uint4(h[0], h[1], h[2], h[3]);
+    *reinterpret_cast<uint4*>(b.act + tc::act_index(b.row, lo + 4 * q)) = make_uint4(l[0], l[1], l[2], l[3]);
+  }
 }
+__device__ __forceinline__ void ld32(const Blk& b, int col, float* v) { ld_row<8>(b, col, v); }
+__device__ __forceinline__ void ld16(const Blk& b, int col, float* v) { ld_row<4>(b, col, v); }
 // 16 / 32 / 8 activations -> hi parts at `hi`, lo parts at `lo`
-__device__ __forceinline__ void st16(const Blk& b, int hi, int lo, const float* v) {
-  uint32_t h[16], l[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) tc::split_tf32(v[j], h[j], l[j]);
-  tc::tmem_st16(b.tAhi + hi, h);
-  tc::tmem_st16(b.tAhi + lo, l);
-}
-__device__ __forceinline__ void st32(const Blk& b, int hi, int lo, const float* v) {
-  st16(b, hi, lo, v);
-  st16(b, hi + 16, lo + 16, v + 16);
-}
-__device__ __forceinline__ void st8(const Blk& b, int hi, int lo, const float* v) {
-  uint32_t h[8], l[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) tc::split_tf32(v[j], h[j], l[j]);
-  tc::tmem_st8(b.tAhi + hi, h);
-  tc::tmem_st8(b.tAhi + lo, l);
-}
+__device__ __forceinline__ void st16(const Blk& b, int hi, int lo, const float* v) { st_split<4>(b, hi, lo, v); }
+__device__ __forceinline__ void st32(const Blk& b, int hi, int lo, const float* v) { st_split<8>(b, hi, lo, v); }
+__device__ __forceinline__ void st8(const Blk& b, int hi, int lo, const float* v) { st_split<2>(b, hi, lo, v); }
 
 template <int G, bool DEBUG>
 __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
@@ -212,14 +217,12 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   uint64_t* const bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* const wfull = bars;
   uint64_t* const wempty = bars + NBUF;
-  uint64_t* const mma_bars = bars + 2 * NBUF;                 // [NBLK]
-  uint32_t* const tmem_base_s = reinterpret_cast<uint32_t*>(bars + 2 * NBUF + NBLK);
-  uint64_t* const res_bar = bars + 2 * NBUF + NBLK + 2;        // resident tensor-core tile has landed
+  uint64_t* const res_bar = bars + 2 * NBUF;                  // resident tensor-core tile has landed
 
   const int rfn = pp.rfn, dn = pp.dn;
   const int N = pp.rn * dn;
   const int n_heads = kp.n_heads;
-  const int stages_per_tile = n_heads + 11;                    // heads, prob_embed x2, base_fc.0 x3, base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
+  const int stages_per_tile = n_heads + 16;                    // Producer::stage_source
   const int n_tiles = kp.n_tiles;                              // tiles of PB points
   const int iters = (n_tiles + int(gridDim.x) * NBLK - 1) / (int(gridDim.x) * NBLK);
   const float* __restrict__ W = pp.w_point;
@@ -227,14 +230,11 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   // ---------------- one-time setup ----------------
   if (tid == 0) {
     for (int i = 0; i < NBUF; ++i) { tc::mbar_init(wfull + i, 1); tc::mbar_init(wempty + i, NBLK); }
-    for (int i = 0; i < NBLK; ++i) tc::mbar_init(mma_bars + i, 1);
     tc::mbar_init(res_bar, 1);
     tc::fence_mbar_init();
-    tc::mbar_arrive_expect_tx(res_bar, (tcl::RD1_SIZE + tcl::HST_SIZE) * 4);
+    tc::mbar_arrive_expect_tx(res_bar, tcl::RD1_SIZE * 4);
     tc::bulk_g2s(smem + OFF_RD1, pp.w_tc + tcl::RD1, tcl::RD1_SIZE * 4, res_bar);
-    for (int i = 0; i < tcl::HST_SIZE; i += 4096) tc::bulk_g2s(smem + OFF_HST + i, pp.w_tc + tcl::HST + i, 4096 * 4, res_bar);
   }
-  if (warp == 0) tc::tmem_alloc<512>(tmem_base_s);
   if (tid < NCOMP) {
     auto cp = [&](float* dst, int src, int n) { for (int i = tid; i < n; i += NCOMP) dst[i] = __ldg(W + src + i); };
     for (int hh = 0; hh < 4; ++hh) {
@@ -255,14 +255,11 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     for (int i = tid; i < 64 * 16; i += NCOMP)
       sWg1[(i & 15) * 64 + own_col<GE>((i >> 4) / CPL, (i >> 4) % CPL)] = __ldg(W + lay::GRP_D2 + lay::GEO1_W + i);
     cp(sWg1 + 64 * 16, lay::GRP_D2 + lay::GEO1_B, 16);
-    if (tid < stages_per_tile) reinterpret_cast<int2*>(smem + OFF_STAB)[tid] = Producer::stage_source(tid, n_heads);
+    if (tid < stages_per_tile) reinterpret_cast<int4*>(smem + OFF_STAB)[tid] = Producer::stage_source(tid, n_heads);
     for (int i = tid; i < 24; i += NCOMP) smem[OFF_CAM + i] = __ldg(pp.que_cam + i);
     for (int i = tid; i < pp.rfn * 20; i += NCOMP) smem[OFF_CAM + 32 + i] = __ldg(pp.view_params + i);
   }
-  tc::fence_before_thread_sync();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem_base = *tmem_base_s;
   tc::mbar_wait(res_bar, 0);
   if (tid < 8) {   // neuray_fc.0 rides on prob_embed.2's MMA (8 extra output rows): its bias as seen through that layer
     float acc = sw[SW_NF0B + tid];
@@ -273,20 +270,17 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 
 #if NR_PRODUCER_WARP
   if (tid >= NCOMP) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_PRODUCER));
     // ---------------- producer warp: a stage goes out the moment its ring slot is free ----------------
     // (fed from a compute thread's issue path, a load only started at that thread's next layer: ~500-850 cycles of every
-    // layer's round trip were the issuing lane waiting for weights, profiles/r2_phase_timing.md)
+    // layer's round trip were the issuing lane waiting for weights)
     if (tid == NCOMP) {
-      const int2* table = reinterpret_cast<const int2*>(smem + OFF_STAB);
+      const int4* table = reinterpret_cast<const int4*>(smem + OFF_STAB);
       const uint32_t total = uint32_t(iters) * uint32_t(stages_per_tile);
       int s = 0;
       for (uint32_t n = 0; n < total; ++n) {
         const uint32_t buf = n % NBUF;
         if (n >= NBUF) tc::mbar_wait(wempty + buf, ((n / NBUF) - 1) & 1);
-        const int2 e = table[s];
-        tc::mbar_arrive_expect_tx(wfull + buf, e.y);
-        tc::bulk_g2s(ring + buf * RING_STAGE, pp.w_tc + e.x, e.y, wfull + buf);
+        load_stage(ring + buf * RING_STAGE, pp.w_tc, table[s], wfull + buf);
         if (++s == stages_per_tile) s = 0;
       }
     }
@@ -294,9 +288,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   } else
 #endif
   {
-#if NR_PRODUCER_WARP
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_COMPUTE));
-#endif
     // ---------------- compute warps ----------------
     const int fh = pp.fh, fw = pp.fw, h = pp.h, w = pp.w;
     const bool feat_align = (fh == h && fw == w);
@@ -316,23 +307,17 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     Blk b;
     b.blk = warp >> 2;
     b.leader = (tid & 127) == 0;
-    b.issuer_warp = (__shfl_sync(0xffffffffu, warp, 0) & 3) == 0;
-    {
-      const uint32_t col0 = tmem_base + TCOLS * b.blk;
-      const uint32_t lane_off = uint32_t((warp & 3) * 32) << 16;
-      b.mAhi = col0; b.mAlo = col0; b.mD = col0;                 // pm3 helpers address columns relative to the block base
-      b.tAhi = col0 + lane_off; b.tAlo = b.tAhi; b.tD = b.tAhi;
-    }
-    b.mma_bar = mma_bars + b.blk;
+    b.act = smem + OFF_ACT + ACT * b.blk;
+    b.act_addr = tc::smem_u32(b.act);
+    b.row = tid & 127;
     b.wfull = wfull; b.wempty = wempty;
     b.ring_addr = tc::smem_u32(ring);
-    b.phase = 0;
     b.wi = 0;
     b.tk = nullptr;
     Producer prod;
     prod.w_tc = pp.w_tc; prod.ring = ring; prod.wfull = wfull; prod.wempty = wempty;
     prod.next = 0; prod.total = uint32_t(iters) * uint32_t(stages_per_tile);
-    prod.stages_per_tile = stages_per_tile; prod.s = 0; prod.table = reinterpret_cast<const int2*>(smem + OFF_STAB);
+    prod.stages_per_tile = stages_per_tile; prod.s = 0; prod.table = reinterpret_cast<const int4*>(smem + OFF_STAB);
 #if NR_PRODUCER_WARP
     b.prod = nullptr;
     (void)prod;
@@ -556,7 +541,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #if NR_GATHER_OVERLAP
         issue_layer<32, 4, 0, 64, 4, 0, 128, 0, 1, 0, 1024 * 4, 0, true, false, false>(b);          // L0: A[0:32]
         if (hd < 2) { g_consume(2 * GSTEP * hd); g_issue(2 * GSTEP * hd + GSTEP, 32); }
-        wait_layer(b);
 #else
         run_layer<32, 4, 0, 4, 0, 0, 1024 * 4, 0, true, false>(b);              // L0: A[0:32]
 #endif
@@ -575,7 +559,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
           if (hd == 0) g_issue(2 * GSTEP, 32);
           else __syncwarp();                                                         // img_feats complete in the buffer
         }
-        wait_layer(b);
 #else
         run_layer<32, 4, 32, 4, 0, 2048 * 4, 3072 * 4, 0, false, true>(b);      // L1: A[32:64]
 #endif
@@ -640,7 +623,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       PM_TICK(5)
       // prob_embed.2 with neuray_fc.0 behind it: N = 48, accumulator columns [96,144)
       issue_layer<48, 4, 0, 64, 4, 0, 96, 0, 1, 0, 1536 * 4, 0, true, true, false>(b);
-      wait_layer(b);
       float gate;
       {
         float x[32];
@@ -653,7 +635,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) gate = fmaf(sw[SW_NF1W + j], elu(h8[j] + sw[SW_NF0C + j]), gate);
       }
-      // base_fc.0, K round A: the neuray_feat inputs (B chunks 5..8), accumulator columns [96,160); completes under ray_dir_fc
+      // base_fc.0, K round A: the neuray_feat inputs (B chunks 5..8), accumulator columns [96,160)
       issue_layer<64, 4, 0, 64, 4, 0, 96, 5, 3, 0, 2048 * 4, 0, true, false, false>(b);
       float rf[40];                                                                  // rgb_feat (35) + zero padding
       {
@@ -664,11 +646,9 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
             const float* __restrict__ w0 = sw + SW_RD0W;
             h16[j] = elu(fmaf(w0[48 + j], dd[3], fmaf(w0[32 + j], dd[2], fmaf(w0[16 + j], dd[1], fmaf(w0[j], dd[0], sw[SW_RD0B + j])))));
           }
-          wait_layer(b);                                                             // round A has read neuray_feat: A is free again
           st16(b, 48, 64, h16);                                                      // ray_dir_fc.2 operand: hi [48,64), lo [64,80)
         }
-        issue_layer_resident<48, 2, 48, 16, 0, 0, 1536 * 4, 0, false>(b, tc::smem_u32(smem + OFF_RD1), b.issuer_warp);   // ray_dir_fc.2: K = 16, accumulator [0,48)
-        wait_layer(b);
+        issue_layer_resident<48, 2, 48, 16, 0, 0, 1536 * 4, 0, false>(b, tc::smem_u32(smem + OFF_RD1));   // ray_dir_fc.2: K = 16, accumulator [0,48)
         ld32(b, 0, rf);
         {
           float t16[16];
@@ -698,7 +678,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         st32(b, 0, 48, rf);                                                          // rgb_feat: hi [0,40), lo [48,88)
         st8(b, 32, 80, rf + 32);
       }
-      // base_fc.0, K round B: rgb_feat (B chunks 0..4); completes under the first butterflies of the view pooling
+      // base_fc.0, K round B: rgb_feat (B chunks 0..4)
       issue_layer<64, 5, 0, 48, 5, 0, 96, 0, 3, 0, 2048 * 4, 0, false, true, true>(b);
       if (DEBUG && kp.dbg != nullptr && row_ok) {
         float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
@@ -710,7 +690,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       // ---------------- view pooling #1 (ibrnet.py:336-339) -> five more K rounds of base_fc.0 ----------------
       // Every lane of a point ends a round with the point's statistics, which is exactly its row of the view-invariant
       // operand: 8 features x (mean0, var0, mean1, var1) = K 32 per round go to A[0:32) and are multiplied into the same
-      // accumulator.  The previous round's MMAs finish under this round's reduction.  The sums over the views go through the
+      // accumulator, B from one ring stage per round.  The sums over the views go through the
       // warp's transposition buffer (pool_rows); the variance comes from the weighted second moment:
       //   sum_v w (x - mu)^2 = sum_v w x^2 - mu^2 (2 - sum_v w),  mu = sum_v w x   (the reference's mean is NOT normalised)
       const float msum = gsum(mrow);
@@ -718,8 +698,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       const float w0 = sigmoidf_(gate) * w1;
       {
         const float c1 = 2.f - gsum(w1), c0 = 2.f - gsum(w0);
-        const uint32_t hst = tc::smem_u32(smem + OFF_HST);
-        const int wq = __shfl_sync(0xffffffffu, warp, 0) & 3;
         auto round = [&](auto rc) {
           constexpr int R = decltype(rc)::value;
           float in[32], st[32];
@@ -735,9 +713,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
             st[8 + i] = fmaf(-st[i] * st[i], c0, st[8 + i]);
             st[24 + i] = fmaf(-st[16 + i] * st[16 + i], c1, st[24 + i]);
           }
-          wait_layer(b);                                                             // the MMAs reading A[0:96) have completed
           st32(b, 0, 32, st);
-          issue_layer_resident<64, 4, 0, 32, 96, 4 * R, 10240 * 4, 2048 * 4, true>(b, hst, wq == (R & 3));
+          issue_layer<64, 4, 0, 32, 4, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, true>(b);
         };
         round(std::integral_constant<int, 0>{}); round(std::integral_constant<int, 1>{}); round(std::integral_constant<int, 2>{});
         round(std::integral_constant<int, 3>{}); round(std::integral_constant<int, 4>{});
@@ -745,7 +722,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 
       PM_TICK(7)
       // ---------------- base_fc on the tensor cores ----------------
-      wait_layer(b);
 #pragma unroll
       for (int c0 = 0; c0 < 64; c0 += 32) {
         float x[32];
@@ -872,7 +848,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
           gpool32(in, st);
 #pragma unroll
           for (int i = 0; i < 16; ++i) st[16 + i] = fmaf(-st[i] * st[i], c2, st[16 + i]);
-          if (R > 0) wait_layer(b);                                                  // the previous round has read A[0:64)
           st32(b, 0, 32, st);
           issue_layer<64, 4, 0, 32, 4, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, (R > 0)>(b);
         };
@@ -882,11 +857,9 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #pragma unroll
           for (int i = 0; i < 8; ++i) st[i] = 0.f;
           st[0] = wmean; st[1] = 1.f;
-          wait_layer(b);
           st8(b, 0, 32, st);
           issue_layer<64, 1, 0, 32, 1, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, true>(b);
         }
-        wait_layer(b);
         // all G rows of a point hold the same 64 hidden pre-activations; lane v keeps columns [v*CPL, (v+1)*CPL)
         float hh[CPL];
         {
@@ -929,10 +902,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     }
   }
 
-  // ---------------- teardown ----------------
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<512>(tmem_base);
 }
 
 }  // namespace pm3

@@ -1,8 +1,11 @@
-// tcgen05 / TMEM / mbarrier primitives for the tensor-core MLP layers (sm_100a, cta_group::1).
+// wgmma / TMA / mbarrier primitives for the tensor-core MLP layers (sm_90a).
 //
-// Layer shape used throughout:  D[128 x N] (fp32, TMEM) += A[128 x K] (tf32, TMEM) * B[N x K]^T (tf32, smem)
-//   * A lives in TMEM: lane = row, one 32-bit column per k (what a thread-per-row producer writes with
-//     tcgen05.st.32x32b); one MMA consumes 8 columns (K = 8 for tf32)
+// Layer shape used throughout:  D[128 x N] (fp32) += A[128 x K] (tf32, smem) * B[N x K]^T (tf32, smem), issued by one
+// warp group (128 threads) as two m64nNk8 wgmma per K = 8 step (rows 0..63 and 64..127)
+//   * A lives in a per-block shared-memory activation tile: row r = the row thread r of the warp group owns, one fp32 column
+//     per k, 32-column slabs of 128 rows in the K-major SWIZZLE_128B layout (act_index).  A thread writes and reads its own
+//     row with 128-bit accesses, which are conflict-free in that layout.  The accumulator of a layer is written back into
+//     columns of the same tile, so the row owners read their outputs the way they read their inputs.
 //   * B lives in shared memory, K-major, 128-byte swizzle: row n = 32 consecutive k (128 B), 8-row atoms of
 //     1024 B; a K = 8 step advances the descriptor start address by 32 B inside the atom
 //   * fp32 accuracy comes from the 3xTF32 split: x = hi + lo with hi = x & 0xffffe000 (exactly representable in
@@ -17,21 +20,7 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-// ---- TMEM allocation (one warp executes these, .sync.aligned) ----
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  static_assert(COLS == 32 || COLS == 64 || COLS == 128 || COLS == 256 || COLS == 512, "power of two >= 32");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-__device__ __forceinline__ void fence_before_thread_sync() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void fence_after_thread_sync() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-// generic-proxy shared-memory writes -> visible to the async proxy (UMMA operand reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // ---- mbarrier ----
@@ -57,11 +46,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   for (uint32_t it = 0; !mbar_try_wait(bar, parity); ++it)
     if (it > (1u << 26)) __trap();
 }
-// all MMAs issued so far by this thread -> one arrival on `bar` when they have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
-
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -77,80 +61,115 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 // named barrier among `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
-// one lane of a fully converged warp (elect.sync)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred px;\n\t"
-      "elect.sync _|px, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, px;\n\t"
-      "}\n"
-      : "=r"(pred)::"memory");
-  return pred != 0;
-}
-
 // ---- descriptors ----
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B, 8-row atoms 1024 B apart (cute::UMMA::SmemDescriptor)
+// shared-memory matrix descriptor, K-major, SWIZZLE_128B, 8-row atoms 1024 B apart (sm_90 GMMA descriptor)
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= uint64_t((saddr & 0x3ffff) >> 4);          // start address, bits [0,14)
   d |= uint64_t(1) << 16;                         // leading byte offset (unused for swizzled K-major), bits [16,30)
   d |= uint64_t(1024 >> 4) << 32;                 // stride byte offset = 1024 B between 8-row atoms, bits [32,46)
-  d |= uint64_t(1) << 46;                         // descriptor version 1 (sm_100)
-  d |= uint64_t(2) << 61;                         // layout type SWIZZLE_128B
+  d |= uint64_t(1) << 62;                         // layout type SWIZZLE_128B, bits [62,64)
   return d;
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): tf32 x tf32 -> f32, A and B K-major, M = 128
-__host__ __device__ constexpr uint32_t idesc_tf32(int N) {
-  return (1u << 4) /* c = f32 */ | (2u << 7) /* a = tf32 */ | (2u << 10) /* b = tf32 */ | (uint32_t(N >> 3) << 17) | (uint32_t(128 >> 4) << 24);
+
+// float index inside a K-major SWIZZLE_128B tile of 32-wide fp32 rows: element (row n, k in [0,32))
+__host__ __device__ constexpr int sw128_index(int n, int k) { return (n >> 3) * 256 + (n & 7) * 32 + ((((k >> 2) ^ (n & 7)) << 2) | (k & 3)); }
+
+// ---- the activation tile: 128 rows, 32-column slabs of 4096 floats (16 KB, 1024-byte aligned) ----
+__host__ __device__ constexpr int act_index(int r, int c) { return (c >> 5) * 4096 + sw128_index(r, c & 31); }
+// A operand of the K = 8 step that starts at column `col` (a multiple of 8), rows 64 * half .. 64 * half + 63
+__device__ __forceinline__ uint64_t act_desc(uint32_t act_saddr, int col, int half) {
+  return smem_desc_sw128(act_saddr + uint32_t((col >> 5) * 16384 + half * 8192 + (col & 31) * 4));
 }
 
-// D[tmem] (+)= A[tmem] * B[smem desc]; issued by ONE thread
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+// ---- wgmma (one warp group) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+
+// d[N/2] (this thread's part of a 64 x N fp32 accumulator) += A[64 x 8] * B[N x 8]^T, both operands in shared memory
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b);
+
+#define NR_WGMMA_D8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[8], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(uint32_t(accumulate))
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n}\n"
+      : NR_WGMMA_D8(0)
+      : "l"(a), "l"(b), "r"(1)
       : "memory");
 }
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n}\n"
+      : NR_WGMMA_D8(0), NR_WGMMA_D8(8)
+      : "l"(a), "l"(b), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<48>(float (&d)[24], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1;\n}\n"
+      : NR_WGMMA_D8(0), NR_WGMMA_D8(8), NR_WGMMA_D8(16)
+      : "l"(a), "l"(b), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n}\n"
+      : NR_WGMMA_D8(0), NR_WGMMA_D8(8), NR_WGMMA_D8(16), NR_WGMMA_D8(24)
+      : "l"(a), "l"(b), "r"(1)
+      : "memory");
+}
+#undef NR_WGMMA_D8
 
-// ---- TMEM <-> registers: 32 lanes x 32-bit, N consecutive columns per thread (thread i of the warp <-> lane base+i) ----
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                 "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr)
-               : "memory");
+// The accumulator fragment of thread t of the warp group <-> the activation tile: for half h and 8-column group j,
+// d[h][4j + {0,1}] = (row 64h + 16 (t / 32) + (t % 32) / 4, columns dcol + 8j + 2 (t % 4) + {0,1}), d[h][4j + {2,3}] = 8 rows lower.
+template <int N>
+__device__ __forceinline__ void acc_load(const float* act, int dcol, int t, float (&d)[2][N / 2]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int h = 0; h < 2; ++h) {
+    const int r = 64 * h + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = dcol + 8 * j + 2 * (t & 3);
+      const float2 x = *reinterpret_cast<const float2*>(act + act_index(r, c));
+      const float2 y = *reinterpret_cast<const float2*>(act + act_index(r + 8, c));
+      d[h][4 * j] = x.x; d[h][4 * j + 1] = x.y; d[h][4 * j + 2] = y.x; d[h][4 * j + 3] = y.y;
+    }
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};\n" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-               "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-               : "memory");
+template <int N>
+__device__ __forceinline__ void acc_store(float* act, int dcol, int t, const float (&d)[2][N / 2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = 64 * h + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int c = dcol + 8 * j + 2 * (t & 3);
+      *reinterpret_cast<float2*>(act + act_index(r, c)) = make_float2(d[h][4 * j], d[h][4 * j + 1]);
+      *reinterpret_cast<float2*>(act + act_index(r + 8, c)) = make_float2(d[h][4 * j + 2], d[h][4 * j + 3]);
+    }
+  }
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};\n" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
 
 // 3xTF32 split
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xffffe000u;
   lo = __float_as_uint(x - __uint_as_float(hi));
 }
-
-// float index inside a K-major SWIZZLE_128B tile of 32-wide fp32 rows: element (row n, k in [0,32))
-__host__ __device__ constexpr int sw128_index(int n, int k) { return (n >> 3) * 256 + (n & 7) * 32 + ((((k >> 2) ^ (n & 7)) << 2) | (k & 3)); }
 
 }  // namespace tc
 }  // namespace nr

@@ -1,6 +1,6 @@
-// Self-test of the tcgen05 layer primitive in nr_tc.cuh: D[128 x N] = A[128 x K] * W[N x K]^T with A in TMEM,
-// W in shared memory (K-major, 128B swizzle), fp32 accumulators in TMEM.  mode 0: single TF32 pass, mode 1: 3xTF32.
-// tests/test_tc_gpu.py compares against an fp64 reference.
+// Self-test of the wgmma layer primitive in nr_tc.cuh: D[128 x N] = A[128 x K] * W[N x K]^T with A in the shared-memory
+// activation tile, W in shared memory (K-major, 128B swizzle), fp32 accumulators in registers written back into the tile.
+// mode 0: single TF32 pass, mode 1: 3xTF32.  tests/test_tc_gpu.py compares against an fp64 reference.
 #include "nr_common.cuh"
 #include "nr_tc.cuh"
 
@@ -12,18 +12,13 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
   static_assert(K % 32 == 0 && N % 16 == 0, "shape");
   constexpr int KS = K / 32;                       // 32-wide K slabs of the B tile
   constexpr int SLAB = N * 32;                     // floats per slab
+  constexpr int COLS = 2 * K + 64;                 // activation tile: A_hi K | A_lo K | D N (<= 64)
   __shared__ __align__(1024) float sBhi[KS * SLAB];
   __shared__ __align__(1024) float sBlo[KS * SLAB];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
-  constexpr int COLS = 256;                        // A_hi K | A_lo K | D N  (<= 64+64+64)
-  const int tid = threadIdx.x, warp = tid >> 5;
+  extern __shared__ __align__(1024) float act[];   // COLS / 32 slabs of 4096 floats
+  const int tid = threadIdx.x;
+  const int cA_hi = 0, cA_lo = K, cD = 2 * K;
 
-  if (warp == 0) tc::tmem_alloc<COLS>(&tmem_base_s);
-  if (tid == 0) {
-    tc::mbar_init(&bar, 1);
-    tc::fence_mbar_init();
-  }
   // weights -> swizzled smem tiles (hi / lo)
   for (int i = tid; i < N * K; i += 128) {
     const int n = i / K, k = i % K;
@@ -33,60 +28,45 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
     sBhi[idx] = __uint_as_float(hi);
     sBlo[idx] = __uint_as_float(lo);
   }
-  tc::fence_proxy_async_smem();
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t lane_base = uint32_t((warp & 3) * 32) << 16;
-  const uint32_t tA_hi = tbase, tA_lo = tbase + K, tD = tbase + 2 * K;
-
-  // this thread's row of A -> TMEM (hi and lo)
+  // this thread's row of A -> the activation tile (hi and lo)
   {
     const float* __restrict__ row = A + size_t(tid) * K;
 #pragma unroll
-    for (int c = 0; c < K; c += 16) {
-      uint32_t hi[16], lo[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) tc::split_tf32(row[c + j], hi[j], lo[j]);
-      tc::tmem_st16(tA_hi + lane_base + c, hi);
-      tc::tmem_st16(tA_lo + lane_base + c, lo);
+    for (int c = 0; c < K; ++c) {
+      uint32_t hi, lo;
+      tc::split_tf32(row[c], hi, lo);
+      act[tc::act_index(tid, cA_hi + c)] = __uint_as_float(hi);
+      act[tc::act_index(tid, cA_lo + c)] = __uint_as_float(lo);
     }
-    tc::tmem_st_wait();
   }
-  tc::fence_before_thread_sync();
+  tc::fence_proxy_async_smem();
   __syncthreads();
 
-  if (tid == 0) {
-    tc::fence_after_thread_sync();
-    const uint32_t idesc = tc::idesc_tf32(N);
+  {
+    const uint32_t sa = tc::smem_u32(act);
+    float d[2][N / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
     const int passes = mode == 0 ? 1 : 3;
-    bool acc = false;
+    tc::wgmma_fence();
     for (int ps = 0; ps < passes; ++ps) {
-      const uint32_t a_t = (ps == 1) ? tA_lo : tA_hi;
+      const int a_c = (ps == 1) ? cA_lo : cA_hi;
       const float* b_s = (ps == 2) ? sBlo : sBhi;
 #pragma unroll
       for (int s = 0; s < K / 8; ++s) {
-        const uint32_t baddr = tc::smem_u32(b_s + (s >> 2) * SLAB) + (s & 3) * 32;
-        tc::mma_tf32_ts(tD, a_t + 8 * s, tc::smem_desc_sw128(baddr), idesc, acc);
-        acc = true;
+        const uint64_t bd = tc::smem_desc_sw128(tc::smem_u32(b_s + (s >> 2) * SLAB) + (s & 3) * 32);
+        tc::wgmma_tf32<N>(d[0], tc::act_desc(sa, a_c + 8 * s, 0), bd);
+        tc::wgmma_tf32<N>(d[1], tc::act_desc(sa, a_c + 8 * s, 1), bd);
       }
     }
-    tc::mma_commit(&bar);
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
+    tc::acc_store<N>(act, cD, tid, d);
   }
-  tc::mbar_wait(&bar, 0);
-  tc::fence_after_thread_sync();
-#pragma unroll
-  for (int c = 0; c < N; c += 16) {
-    float v[16];
-    tc::tmem_ld16(tD + lane_base + c, v);
-    tc::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) D[size_t(tid) * N + c + j] = v[j];
-  }
-  tc::fence_before_thread_sync();
   __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<COLS>(tbase);
+  for (int c = 0; c < N; ++c) D[size_t(tid) * N + c] = act[tc::act_index(tid, cD + c)];
 }
 
 }  // namespace nr
@@ -94,9 +74,14 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
 extern "C" int nr_tc_selftest(const float* A, const float* W, float* D, int n, int k, int mode, void* stream) {
   NR_CHECK_ARG(A && W && D, "null pointer");
   cudaStream_t s = (cudaStream_t)stream;
-  if (n == 32 && k == 32) nr::tc_selftest_kernel<32, 32><<<1, 128, 0, s>>>(A, W, D, mode);
-  else if (n == 64 && k == 64) nr::tc_selftest_kernel<64, 64><<<1, 128, 0, s>>>(A, W, D, mode);
-  else if (n == 16 && k == 64) nr::tc_selftest_kernel<16, 64><<<1, 128, 0, s>>>(A, W, D, mode);
+  auto run = [&](auto* fn, int k_) {
+    const int smem = (2 * k_ + 64) / 32 * 4096 * 4;
+    cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    fn<<<1, 128, smem, s>>>(A, W, D, mode);
+  };
+  if (n == 32 && k == 32) run(nr::tc_selftest_kernel<32, 32>, 32);
+  else if (n == 64 && k == 64) run(nr::tc_selftest_kernel<64, 64>, 64);
+  else if (n == 16 && k == 64) run(nr::tc_selftest_kernel<16, 64>, 64);
   else {
     nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d", n, k);
     return NR_E_UNSUPPORTED;

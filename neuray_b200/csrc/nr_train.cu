@@ -97,7 +97,7 @@ int nr_render_pass_bwd(const NrPassParams* p, const NrBwdParams* b, void* stream
   c.d_hit = b->d_hit_prob;
   c.d_depth = b->d_render_depth;
   cudaStream_t s = (cudaStream_t)stream;
-  auto blocks = [](long long n) { long long g = (n + 127) / 128; return int(g < 148 * 32 ? g : 148 * 32); };
+  auto blocks = [](long long n) { long long g = (n + 127) / 128; return int(g < 132 * 32 ? g : 132 * 32); };
   tr::train_kernel<0><<<blocks(R), 128, 0, s>>>(c, R);      // rows:   gather .. ray_dir_fc
   tr::train_kernel<1><<<blocks(N), 128, 0, s>>>(c, N);      // points: view pooling #1
   tr::train_kernel<2><<<blocks(R), 128, 0, s>>>(c, R);      // rows:   base_fc .. rgb_fc

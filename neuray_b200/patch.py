@@ -1,4 +1,4 @@
-"""Installs the B200 path into an importable reference tree so that its own entry points (render.py,
+"""Installs the native path into an importable reference tree so that its own entry points (render.py,
 run_training.py, eval.py) run unchanged:
 
     import neuray_b200.patch as patch

@@ -195,7 +195,7 @@ def pass_index_map(owner, is_fine, dev):
 def _check_supported(owner):
     cfg = owner.cfg
     if cfg.get("use_dr_prediction", False):
-        raise NotImplementedError("use_dr_prediction (direct rendering / SH fit) is outside the B200 hot path (SURVEY.md 8f)")
+        raise NotImplementedError("use_dr_prediction (direct rendering / SH fit) is outside the native hot path (SURVEY.md 8f)")
 
 
 def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit):

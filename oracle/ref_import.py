@@ -8,9 +8,8 @@ register empty module stubs (with a __spec__, otherwise torch._dynamo's find_spe
 let the reference import.  `IBRNetWithNeuRay.posenc` pins its table to "cuda:0"
 (network/ibrnet.py:312); on a GPU-less box we make that particular `.to("cuda:0")` a no-op.
 
-Nothing in neuray_b200/ may import this file.  Root of the reference tree: $NEURAY_REFERENCE_ROOT, else /root/reference
-(the build container), else baseline/_ref (the verbatim copy made by baseline/install_ref.py, which travels to the GPU
-box).  `inplace_abn` (ABN / InPlaceABN = batch-norm + leaky_relu(0.01), loads network/mvsnet/mvsnet_pl.ckpt strictly)
+Nothing in neuray_b200/, tests/ or bench.py may import this file: only the golden generators under oracle/ do.  Root of the
+reference tree: $NEURAY_REFERENCE_ROOT, else /root/reference.  `inplace_abn` (ABN / InPlaceABN = batch-norm + leaky_relu(0.01), loads network/mvsnet/mvsnet_pl.ckpt strictly)
 and `kornia.utils.create_meshgrid` get functional stand-ins because CostVolumeInitNet / MVSNet really call them.
 """
 import importlib.machinery
@@ -18,17 +17,8 @@ import os
 import sys
 import types
 
-_REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
 def _find_root():
-    env = os.environ.get("NEURAY_REFERENCE_ROOT")
-    if env:
-        return env
-    for cand in ("/root/reference", os.path.join(_REPO, "baseline", "_ref")):
-        if os.path.isdir(os.path.join(cand, "network")):
-            return cand
-    return "/root/reference"
+    return os.environ.get("NEURAY_REFERENCE_ROOT", "/root/reference")
 
 
 REFERENCE_ROOT = _find_root()

@@ -102,8 +102,8 @@ static void host_conv(const ConvP& p) {
 struct HostOps {
   template <int BM, int BN>
   static void conv_k(const ConvP& p) { p.Cin % 32 == 0 ? host_conv<BM, BN, 32>(p) : host_conv<BM, BN, 16>(p); }
-  void conv(const ConvP& p) {       // the launcher's dispatch (csrc/nr_encoder.cu launch_conv), 148 SMs assumed for the automatic choice
-    const int bm = p.bm != 0 ? p.bm : pick_bm(p.Cout, (long long)p.N * p.Ho * p.Wo, 148);
+  void conv(const ConvP& p) {       // the launcher's dispatch (csrc/nr_encoder.cu launch_conv), 132 SMs (H100) assumed for the automatic choice
+    const int bm = p.bm != 0 ? p.bm : pick_bm(p.Cout, (long long)p.N * p.Ho * p.Wo, 132);
     switch (p.Cout) {
       case 32: bm == 256 ? conv_k<256, 32>(p) : conv_k<128, 32>(p); break;
       case 64: bm == 64 ? conv_k<64, 64>(p) : conv_k<128, 64>(p); break;

@@ -26,7 +26,7 @@ def harness():
     src = os.path.join(ROOT, "tests", "cpu_harness", "train_cpu_harness.cu")
     deps = [src, os.path.join(ROOT, "neuray_b200", "csrc", "nr_train_math.cuh"), os.path.join(ROOT, "neuray_b200", "csrc", "nr_common.cuh")]
     if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O1", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O1", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                         "-o", so, src], check=True, capture_output=True)
     lib = C.CDLL(so)
     lib.nr_train_cpu.restype = C.c_int

@@ -72,7 +72,7 @@ def harness():
     lib = os.path.join(BUILD, "libloss_cpu_harness.so")
     deps = [src] + [os.path.join(ROOT, "neuray_b200", "csrc", f) for f in ("nr_loss_math.cuh", "nr_train_math.cuh", "nr_common.cuh")]
     if not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps):
-        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O1", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O1", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                         src, "-o", lib], check=True)
     return C.CDLL(lib)
 

@@ -49,7 +49,7 @@ def harness():
     lib = os.path.join(BUILD, "libmvs_cpu_harness.so")
     deps = [src] + [os.path.join(ROOT, "neuray_b200", "csrc", f) for f in ("nr_mvs.cuh", "nr_mvs_graph.cuh", "nr_encoder_graph.cuh", "nr_conv.cuh")]
     if not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps):
-        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                         src, "-o", lib], check=True)
     return C.CDLL(lib)
 
@@ -102,7 +102,7 @@ def conv_harness():
     lib = os.path.join(BUILD, "libconv_cpu_harness.so")
     deps = [src] + [os.path.join(ROOT, "neuray_b200", "csrc", f) for f in ("nr_conv.cuh", "nr_encoder_graph.cuh", "nr_common.cuh")]
     if not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps):
-        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.run(["nvcc", "-shared", "-Xcompiler", "-fPIC", "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                         src, "-o", lib], check=True)
     return C.CDLL(lib)
 

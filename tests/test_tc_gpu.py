@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 layer primitive (A in TMEM, W in swizzled smem, fp32 accumulate in TMEM) against fp64 matmul."""
+"""GPU: the wgmma layer primitive (A in the shared-memory activation tile, W in swizzled smem, fp32 accumulate) against fp64 matmul."""
 import pytest
 import torch
 

@@ -51,7 +51,7 @@ for blk in (0, 1):
     print(f"block {blk}: tile (16 points x 8 views = 128 rows) total {tot:.0f} cycles")
     print("  " + "  ".join(f"{nm[i]}:{d[i]:.0f}" for i in range(15)))
 # one layer's round trip (vis_fc.0): stamps 16.. = entry, st-wait+fence, barrier, weights there (issuer), MMAs issued + committed,
-# MMA completion seen, accumulator loaded (tcgen05.ld + wait), epilogue computed, next operand stored (tcgen05.st issued)
+# MMA completion seen, accumulator loaded (wgmma wait + store into the tile), epilogue computed, next operand stored (stored into the tile)
 lbl = ["st-wait+fence", "barrier", "wfull wait", "issue+commit", "mma wait", "ld32", "epilogue math", "st32 issue"]
 for blk in (0, 1):
     m = t[4:40, blk, 16:25].double()
