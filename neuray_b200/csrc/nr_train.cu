@@ -40,7 +40,7 @@ static const SlotName kSlots[] = {
     {"R_SLOTS", R_SLOTS}, {"G_SLOTS", G_SLOTS}, {"P_SLOTS", P_SLOTS}, {"GP_SLOTS", GP_SLOTS},
     {"R_RF", R_RF}, {"R_DD", R_DD}, {"R_H1", R_H1}, {"R_H2", R_H2}, {"R_P1", R_P1}, {"R_RGBF", R_RGBF}, {"R_NF", R_NF}, {"R_Q8", R_Q8},
     {"R_R16", R_R16}, {"R_B1", R_B1}, {"R_U", R_U}, {"R_VH", R_VH}, {"R_X2", R_X2}, {"R_U2", R_U2}, {"R_WH", R_WH}, {"R_CH1", R_CH1},
-    {"R_CH2", R_CH2}, {"R_MASK", R_MASK}, {"R_HITN", R_HITN}, {"R_VISN", R_VISN}, {"R_BLEND", R_BLEND},
+    {"R_CH2", R_CH2}, {"R_MASK", R_MASK}, {"R_HITN", R_HITN}, {"R_VISN", R_VISN}, {"R_BLEND", R_BLEND}, {"R_TCODE", R_TCODE},
     {"G_DD0", G_DD0}, {"G_DD1", G_DD1}, {"G_DD2", G_DD2}, {"G_PE0", G_PE0}, {"G_PE1", G_PE1}, {"G_NF0", G_NF0}, {"G_NF1", G_NF1},
     {"G_RD0", G_RD0}, {"G_RD1", G_RD1}, {"G_B0", G_B0}, {"G_B1", G_B1}, {"G_V0", G_V0}, {"G_V1", G_V1}, {"G_V20", G_V20}, {"G_V21", G_V21},
     {"G_C0", G_C0}, {"G_C1", G_C1}, {"G_C2", G_C2},

@@ -229,6 +229,45 @@ def test_hand_written_backward_matches_the_reference_gradients(harness, name):
 
 
 @pytest.mark.parametrize("name", ["train8", "views10"])
+def test_float64_restatement_matches_the_reference_gradients(name):
+    """The float64 restatement (tests/torch_restatement.py, autograd, every input cast to double) -- the reference the GPU
+    backward is judged by in tests/test_backward_gpu.py -- against the unmodified reference's gradients on the golden
+    case's stage rays, at the tolerance of the test above."""
+    import numpy as np
+    from golden_io import GOLDEN_DIR, GoldenCase
+    g = GoldenCase(name)
+    z = np.load(os.path.join(GOLDEN_DIR, f"grads_{name}.npz"))
+    lw = {k[3:]: torch.from_numpy(z[k]).double() for k in z.files if k.startswith("lw_")}
+    gold = {k[5:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("grad_")}
+    sel = g.stage_sel
+    d = lambda t: t.double()
+    coords = d(g.que["coords"][:, sel])
+    use_vis = g.cfg.get("dist_decoder_cfg", {}).get("use_vis", True)
+    ref = {k: d(g.ref[k]) for k in ("poses", "Ks", "depth_range", "imgs")}
+    ref["ray_feats"] = d(g.ref["ray_feats"]).requires_grad_(True)
+    ref["img_feats"] = d(g.ref["img_feats"]).requires_grad_(True)
+    checked = 0
+    for dec, agg, depth, gp, gh, gd in (("dist_decoder", "agg_net", g.que_depth[:, sel], lw["gw_c"], lw["gh_c"], None),
+                                        ("fine_dist_decoder", "fine_agg_net", g.que_depth_fine[:, sel], lw["gw_f"], None, lw["gd_f"])):
+        P = {k: d(v).requires_grad_(True) for k, v in g.W.items() if k.startswith(dec + ".") or k.startswith(agg + ".")}
+        cfgv = {"use_vis_prob": use_vis, "var_bias": g.cfg.get(dec + "_cfg", {}).get("bias_val", 0.05)}
+        pix, hit, dep = autograd_path.render_pass_torch(P, dec, agg, cfgv, d(depth), coords, d(g.que["poses"]), d(g.que["Ks"]),
+                                                        d(g.que["depth_range"]), ref, d(weights.posenc_table(depth.shape[-1])))
+        loss = (pix * gp).sum() + ((hit * gh).sum() if gh is not None else 0.0) + ((dep * gd).sum() if gd is not None else 0.0)
+        loss.backward()
+        for k, p in P.items():
+            if k not in gold:
+                assert p.grad is None or float(p.grad.abs().max()) == 0.0, k
+                continue
+            err, scale = float((p.grad - gold[k].double()).abs().max()), float(gold[k].abs().max())
+            assert err <= 3e-4 * max(scale, 1e-3) + 3e-6, (k, err, scale)
+            checked += 1
+    assert checked == len([k for k in gold if not k.startswith("ref_")])
+    for got, ref_g in ((ref["ray_feats"].grad, gold["ref_ray_feats"]), (ref["img_feats"].grad, gold["ref_img_feats"])):
+        assert float((got - ref_g.double()).abs().max()) <= 3e-4 * float(ref_g.abs().max()) + 3e-6
+
+
+@pytest.mark.parametrize("name", ["train8", "views10"])
 def test_self_hit_prob_matches_the_reference(harness, name):
     """predict_self_hit_prob as the unmodified reference computes it (values and autograd gradients stored in
     tests/golden/grads_*.npz) against nr_self_hit_prob's routine (host build) and against the oracle."""
