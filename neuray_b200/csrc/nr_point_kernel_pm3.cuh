@@ -104,6 +104,8 @@ __device__ __forceinline__ void issue_layer(Blk& b) {
     dhi[s] = tc::smem_desc_sw128(base + OFF_HI);
     dlo[s] = tc::smem_desc_sw128(base + OFF_LO);
   }
+  tc::wgmma_fence_operand(d[0]);
+  tc::wgmma_fence_operand(d[1]);
   tc::wgmma_fence();
 #pragma unroll
   for (int ps = 0; ps < 3; ++ps) {
@@ -120,8 +122,11 @@ __device__ __forceinline__ void issue_layer(Blk& b) {
     }
   }
   tc::wgmma_commit();
-  tc::wgmma_wait_all();
   if (b.tk) b.tk[4] = clock64();
+  tc::wgmma_wait_all();
+  tc::wgmma_fence_operand(d[0]);
+  tc::wgmma_fence_operand(d[1]);
+  if (b.tk) b.tk[5] = clock64();
   tc::acc_store<N>(b.act, DCOL, b.row, d);
   tc::named_sync(2 + b.blk, 128);            // outputs in the tile; every warp's reads of the stages have completed
   if (RELEASE) {
@@ -131,7 +136,7 @@ __device__ __forceinline__ void issue_layer(Blk& b) {
     }
     b.wi += NSTG;
   }
-  if (b.tk) b.tk[5] = clock64();
+  if (b.tk) b.tk[6] = clock64();
 }
 // Same, B operand = a resident shared-memory tile at byte address `base` (hi slabs first, SLAB bytes apart; lo parts
 // OFF_LO bytes further): no ring accounting.
@@ -148,6 +153,8 @@ __device__ __forceinline__ void issue_layer_resident(Blk& b, uint32_t base) {
       for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
   }
   const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + OFF_LO);
+  tc::wgmma_fence_operand(d[0]);
+  tc::wgmma_fence_operand(d[1]);
   tc::wgmma_fence();
 #pragma unroll
   for (int ps = 0; ps < 3; ++ps) {
@@ -163,6 +170,8 @@ __device__ __forceinline__ void issue_layer_resident(Blk& b, uint32_t base) {
   }
   tc::wgmma_commit();
   tc::wgmma_wait_all();
+  tc::wgmma_fence_operand(d[0]);
+  tc::wgmma_fence_operand(d[1]);
   tc::acc_store<N>(b.act, DCOL, b.row, d);
   tc::named_sync(2 + b.blk, 128);
 }
@@ -749,7 +758,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       {
         float x[32];
         ld32(b, 128, x);
-        if (b.tk) b.tk[6] = clock64();
+        if (b.tk) b.tk[7] = clock64();
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           const float4 bb = *reinterpret_cast<const float4*>(sw + SW_V0B + 4 * q);
@@ -758,9 +767,9 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
           x[4 * q + 2] = elu(fmaf(w1, x[4 * q + 2], bb.z)); x[4 * q + 3] = elu(fmaf(w1, x[4 * q + 3], bb.w));
           lg = fmaf(wl.w, x[4 * q + 3], fmaf(wl.z, x[4 * q + 2], fmaf(wl.y, x[4 * q + 1], fmaf(wl.x, x[4 * q], lg))));
         }
-        if (b.tk) b.tk[7] = clock64();
+        if (b.tk) b.tk[8] = clock64();
         st32(b, 32, 96, x);
-        if (b.tk) { b.tk[8] = clock64(); b.tk = nullptr; }
+        if (b.tk) { b.tk[9] = clock64(); b.tk = nullptr; }
       }
       PM_TICK(10)
       const float visa = sigmoidf_(elu(lg)) * mrow;

@@ -86,6 +86,15 @@ __device__ __forceinline__ uint64_t act_desc(uint32_t act_saddr, int col, int ha
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+// Operand fence on an accumulator fragment: every register of `d` is defined before this point and read after it.  Put
+// before wgmma_fence() and after the wait that completes the batch.  Without it the compiler may sink the moves that
+// build the accumulators (zeroing, acc_load) past wgmma_fence(), in between the wgmmas; ptxas then injects a
+// warpgroup.arrive there and serialises every wgmma of the function (C7520: each one issued alone and waited for).
+template <int M>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[M]) {
+#pragma unroll
+  for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // d[N/2] (this thread's part of a 64 x N fp32 accumulator) += A[64 x 8] * B[N x 8]^T, both operands in shared memory
 template <int N>

@@ -1,14 +1,14 @@
 // Self-test of the wgmma layer primitive in nr_tc.cuh: D[128 x N] = A[128 x K] * W[N x K]^T with A in the shared-memory
 // activation tile, W in shared memory (K-major, 128B swizzle), fp32 accumulators in registers written back into the tile.
-// mode 0: single TF32 pass, mode 1: 3xTF32.  tests/test_tc_gpu.py compares against an fp64 reference.
+// mode 0: single TF32 pass (PASSES = 1), mode 1: 3xTF32 (PASSES = 3).  tests/test_tc_gpu.py compares against an fp64 reference.
 #include "nr_common.cuh"
 #include "nr_tc.cuh"
 
 namespace nr {
 
-template <int N, int K>
+template <int N, int K, int PASSES>
 __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ W,
-                                                           float* __restrict__ D, int mode) {
+                                                           float* __restrict__ D) {
   static_assert(K % 32 == 0 && N % 16 == 0, "shape");
   constexpr int KS = K / 32;                       // 32-wide K slabs of the B tile
   constexpr int SLAB = N * 32;                     // floats per slab
@@ -49,9 +49,11 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
-    const int passes = mode == 0 ? 1 : 3;
+    tc::wgmma_fence_operand(d[0]);
+    tc::wgmma_fence_operand(d[1]);
     tc::wgmma_fence();
-    for (int ps = 0; ps < passes; ++ps) {
+#pragma unroll
+    for (int ps = 0; ps < PASSES; ++ps) {
       const int a_c = (ps == 1) ? cA_lo : cA_hi;
       const float* b_s = (ps == 2) ? sBlo : sBhi;
 #pragma unroll
@@ -63,6 +65,8 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
     }
     tc::wgmma_commit();
     tc::wgmma_wait_all();
+    tc::wgmma_fence_operand(d[0]);
+    tc::wgmma_fence_operand(d[1]);
     tc::acc_store<N>(act, cD, tid, d);
   }
   __syncthreads();
@@ -74,14 +78,16 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
 extern "C" int nr_tc_selftest(const float* A, const float* W, float* D, int n, int k, int mode, void* stream) {
   NR_CHECK_ARG(A && W && D, "null pointer");
   cudaStream_t s = (cudaStream_t)stream;
-  auto run = [&](auto* fn, int k_) {
+  auto run = [&](auto* fn1, auto* fn3, int k_) {
+    // the pass count is a template argument: a runtime loop around the wgmma batch makes ptxas serialise it
+    auto* fn = mode == 0 ? fn1 : fn3;
     const int smem = (2 * k_ + 64) / 32 * 4096 * 4;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    fn<<<1, 128, smem, s>>>(A, W, D, mode);
+    fn<<<1, 128, smem, s>>>(A, W, D);
   };
-  if (n == 32 && k == 32) run(nr::tc_selftest_kernel<32, 32>, 32);
-  else if (n == 64 && k == 64) run(nr::tc_selftest_kernel<64, 64>, 64);
-  else if (n == 16 && k == 64) run(nr::tc_selftest_kernel<16, 64>, 64);
+  if (n == 32 && k == 32) run(nr::tc_selftest_kernel<32, 32, 1>, nr::tc_selftest_kernel<32, 32, 3>, 32);
+  else if (n == 64 && k == 64) run(nr::tc_selftest_kernel<64, 64, 1>, nr::tc_selftest_kernel<64, 64, 3>, 64);
+  else if (n == 16 && k == 64) run(nr::tc_selftest_kernel<16, 64, 1>, nr::tc_selftest_kernel<16, 64, 3>, 64);
   else {
     nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d", n, k);
     return NR_E_UNSUPPORTED;

@@ -50,10 +50,11 @@ for blk in (0, 1):
     tot = (t[4:40, blk, 15] - t[4:40, blk, 0]).double().mean()
     print(f"block {blk}: tile (16 points x 8 views = 128 rows) total {tot:.0f} cycles")
     print("  " + "  ".join(f"{nm[i]}:{d[i]:.0f}" for i in range(15)))
-# one layer's round trip (vis_fc.0): stamps 16.. = entry, st-wait+fence, barrier, weights there (issuer), MMAs issued + committed,
-# MMA completion seen, accumulator loaded (wgmma wait + store into the tile), epilogue computed, next operand stored (stored into the tile)
-lbl = ["st-wait+fence", "barrier", "wfull wait", "issue+commit", "mma wait", "ld32", "epilogue math", "st32 issue"]
+# one layer's round trip (vis_fc.0): stamps 16.. = entry, A columns fenced, barrier, weights there (issuer), accumulators set
+# up + MMAs issued + committed, wgmma wait, accumulators stored + barrier + ring release, outputs loaded, epilogue
+# computed, next operand stored
+lbl = ["fence", "barrier", "wfull wait", "issue+commit", "mma wait", "acc store+barrier", "ld32", "epilogue math", "st32"]
 for blk in (0, 1):
-    m = t[4:40, blk, 16:25].double()
+    m = t[4:40, blk, 16:26].double()
     d = (m[:, 1:] - m[:, :-1]).mean(0)
-    print(f"block {blk} vis_fc.0 round trip: " + "  ".join(f"{lbl[i]}:{d[i]:.0f}" for i in range(8)) + f"  total {float((m[:, 8] - m[:, 0]).mean()):.0f}")
+    print(f"block {blk} vis_fc.0 round trip: " + "  ".join(f"{lbl[i]}:{d[i]:.0f}" for i in range(9)) + f"  total {float((m[:, 9] - m[:, 0]).mean()):.0f}")
