@@ -2,14 +2,15 @@
 // the per-point layers -- reference renderer.py:171-178 up to geometry_fc, ibrnet.py:315-354.  One kernel
 // (nr_point_kernel_pm3.cuh, one 128-row block per SM); this file holds what its pieces share and the launcher:
 //
-//   * thread r of the block's warp group owns (point,view) row r of the 128-row block = row r of its shared-memory
-//     activation tile; row = point * G + view, G = lanes per point
+//   * thread r of each of the block's two compute warp groups works on (point,view) row r of the 128-row block = row r
+//     of its shared-memory activation tile, row = point * G + view (G = lanes per point); the two warp groups split the
+//     row's columns between them (nr_point_kernel_pm3.cuh)
 //   * a layer  D[128 x N] += A[128 x K] * W^T :  A (hi and lo parts of the 3xTF32 split) is written into the activation
 //     tile by the row owners, W^T (hi / lo, pre-split and pre-swizzled by nr_pack_weights) sits in shared memory, the warp
 //     group multiplies them with wgmma and writes D back into the tile for the bias / activation epilogue, whose result
-//     goes back into the tile as the next A
+//     goes back into the tile as the next A; warp group c issues the MMAs of rows 64c .. 64c + 63
 //   * weights stream through a 4 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk); full/empty
-//     mbarriers, the "empty" arrival comes from the block once the consuming wgmma have completed
+//     mbarriers, the "empty" arrival comes from thread 0 once both warp groups' consuming wgmma have completed
 #include <type_traits>
 
 #include "nr_common.cuh"
@@ -37,7 +38,7 @@ static_assert(SW_NF0C + 8 <= SW, "small weights overflow");
 struct KParams {
   NrPassParams p;
   float* dbg;
-  long long* timing;   // optional: clock64() at phase boundaries, CTA 0, threads 0 and 128: [tile][2][32]
+  long long* timing;   // optional: clock64() at phase boundaries, CTA 0, thread 0 of each compute warp group: [tile][2][32]
   int P, n_tiles, n_heads;
 };
 
@@ -48,59 +49,28 @@ __device__ __forceinline__ void load_stage(float* slot, const float* w_tc, int4 
   if (e.w) tc::bulk_g2s(slot + e.y / 4, w_tc + e.z, e.w, full);
 }
 
-// The weight stream, driven by ONE thread (thread 0) from inside its own MMA-issue path: before it waits for a stage it
-// issues every stage up to that one (blocking on the ring slot if it has to) and opportunistically up to NBUF-1 further.
-struct Producer {
-  const float* w_tc;
-  float* ring;
-  uint64_t *wfull, *wempty;
-  const int4* table;      // shared: per stage of a tile (load_stage's copies), built once at kernel start
-  uint32_t next;          // next stage index to issue
-  uint32_t total;         // iters * stages_per_tile
-  int stages_per_tile;
-  int s;                  // next % stages_per_tile, kept as a running counter (this code runs on one lane, inside block 0's MMA-issue
-                          // path: every instruction counts)
-
-  // copies of stage s of a tile: heads, prob_embed x2, base_fc.0 x3, the view-pooled base_fc.0 inputs x5 (hi slab | lo slab
-  // of the resident-layout HST tile), base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
-  __device__ static int4 stage_source(int s, int n_heads) {
-    if (s < n_heads) return make_int4(tcl::HEAD0 + s * RING_STAGE, RING_STAGE * 4, 0, 0);
-    const int t = s - n_heads;
-    if (t >= 5 && t < 10) return make_int4(tcl::HST + (t - 5) * 2048, 2048 * 4, tcl::HST + tcl::HST_SIZE / 2 + (t - 5) * 2048, 2048 * 4);
-    const int src = t == 0 ? tcl::PE0 : t == 1 ? tcl::PE1 : t <= 4 ? tcl::B0 + (t - 2) * RING_STAGE : t == 10 ? tcl::B1 : t == 11 ? tcl::V01
-                  : t == 12 ? tcl::V2R : tcl::G0 + (t - 13) * RING_STAGE;
-    return make_int4(src, t == 1 ? 3072 * 4 : RING_STAGE * 4, 0, 0);
-  }
-  __device__ __forceinline__ void issue() {
-    const uint32_t buf = next % NBUF;
-    load_stage(ring + buf * RING_STAGE, w_tc, table[s], wfull + buf);
-    ++next;
-    if (++s == stages_per_tile) s = 0;
-  }
-  // make sure stages [.., last] are in flight; then try to run ahead without blocking
-  __device__ __forceinline__ void feed(uint32_t last) {
-    while (next <= last && next < total) {
-      if (next >= NBUF) tc::mbar_wait(wempty + (next % NBUF), ((next / NBUF) - 1) & 1);
-      issue();
-    }
-    while (next < total && next <= last + (NBUF - 1)) {
-      if (next >= NBUF && !tc::mbar_try_wait(wempty + (next % NBUF), ((next / NBUF) - 1) & 1)) break;
-      issue();
-    }
-  }
-};
+// copies of stage s of a tile: heads, prob_embed x2, base_fc.0 x3, the view-pooled base_fc.0 inputs x5 (hi slab | lo slab
+// of the resident-layout HST tile), base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
+__device__ __forceinline__ int4 stage_source(int s, int n_heads) {
+  if (s < n_heads) return make_int4(tcl::HEAD0 + s * RING_STAGE, RING_STAGE * 4, 0, 0);
+  const int t = s - n_heads;
+  if (t >= 5 && t < 10) return make_int4(tcl::HST + (t - 5) * 2048, 2048 * 4, tcl::HST + tcl::HST_SIZE / 2 + (t - 5) * 2048, 2048 * 4);
+  const int src = t == 0 ? tcl::PE0 : t == 1 ? tcl::PE1 : t <= 4 ? tcl::B0 + (t - 2) * RING_STAGE : t == 10 ? tcl::B1 : t == 11 ? tcl::V01
+                : t == 12 ? tcl::V2R : tcl::G0 + (t - 13) * RING_STAGE;
+  return make_int4(src, t == 1 ? 3072 * 4 : RING_STAGE * 4, 0, 0);
+}
 
 // Everything a compute thread needs to drive its block's tensor-core layers.
 struct Blk {
   float* act;                   // the block's activation tile (tc::act_index)
   uint32_t act_addr;            // its shared-space byte address
-  int row;                      // this thread's row of the tile = its index in the warp group
+  int row;                      // this thread's row of the tile = its index in its warp group
+  int wg;                       // compute warp group (0, 1): issues the MMAs of rows 64 wg .. 64 wg + 63, owns columns 4 wg + [0,4) of every 8
+  int rbase, key;               // act_index(row, c + 4 wg) = (c >> 5) * 4096 + rbase + ((((c & 31) >> 2) ^ key) << 2) for c % 8 == 0
   uint64_t *wfull, *wempty;     // arrays [NBUF]
   uint32_t ring_addr;           // shared-space byte address of the ring
   uint32_t wi;                  // weight stages consumed so far (same sequence in every thread)
-  int blk;
-  bool leader;
-  Producer* prod;               // non-null in the one thread that also feeds the weight ring (point-major kernel)
+  bool leader;                  // thread 0: releases the ring stages
   long long* tk;                // diagnostics: where run_layer drops clock64() stamps (nullptr: off)
 };
 
@@ -331,9 +301,8 @@ static int launch_pm3(pkt::KParams kp, cudaStream_t stream) {
   const long long N = (long long)kp.p.rn * kp.p.dn;
   kp.P = PB;
   kp.n_tiles = int((N + PB - 1) / PB);
-  const int groups = (kp.n_tiles + pkt::pm3::NBLK - 1) / pkt::pm3::NBLK;
   const int sms = device_sms();
-  const int grid = groups < sms ? groups : sms;
+  const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
   return (kp.dbg || kp.timing) ? launch_pm3_inst<G, true>(kp, grid, stream) : launch_pm3_inst<G, false>(kp, grid, stream);
 }
 

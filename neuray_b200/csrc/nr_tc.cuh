@@ -1,7 +1,8 @@
 // wgmma / TMA / mbarrier primitives for the tensor-core MLP layers (sm_90a).
 //
-// Layer shape used throughout:  D[128 x N] (fp32) += A[128 x K] (tf32, smem) * B[N x K]^T (tf32, smem), issued by one
-// warp group (128 threads) as two m64nNk8 wgmma per K = 8 step (rows 0..63 and 64..127)
+// Layer shape used throughout:  D[128 x N] (fp32) += A[128 x K] (tf32, smem) * B[N x K]^T (tf32, smem), issued as one
+// m64nNk8 wgmma per K = 8 step for each row half (rows 0..63 and 64..127): by two warp groups, one half each (point
+// kernel), or both halves by one warp group (self-test)
 //   * A lives in a per-block shared-memory activation tile: row r = the row thread r of the warp group owns, one fp32 column
 //     per k, 32-column slabs of 128 rows in the K-major SWIZZLE_128B layout (act_index).  A thread writes and reads its own
 //     row with 128-bit accesses, which are conflict-free in that layout.  The accumulator of a layer is written back into
@@ -60,6 +61,16 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 }
 // named barrier among `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
+// arrive on a named barrier without waiting: the shared-memory writes before it are visible to the threads that pass
+// bar.sync on the same barrier
+__device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
+
+// per-thread register budget of the executing warp group (all of its warps execute it): give registers back to the CTA's
+// pool / take them from it
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(R)); }
 
 // ---- descriptors ----
 // shared-memory matrix descriptor, K-major, SWIZZLE_128B, 8-row atoms 1024 B apart (sm_90 GMMA descriptor)
@@ -88,7 +99,7 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
 // Operand fence on an accumulator fragment: every register of `d` is defined before this point and read after it.  Put
 // before wgmma_fence() and after the wait that completes the batch.  Without it the compiler may sink the moves that
-// build the accumulators (zeroing, acc_load) past wgmma_fence(), in between the wgmmas; ptxas then injects a
+// build the accumulators (zeroing, acc_load_half) past wgmma_fence(), in between the wgmmas; ptxas then injects a
 // warpgroup.arrive there and serialises every wgmma of the function (C7520: each one issued alone and waited for).
 template <int M>
 __device__ __forceinline__ void wgmma_fence_operand(float (&d)[M]) {
@@ -144,34 +155,35 @@ __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint6
 }
 #undef NR_WGMMA_D8
 
-// The accumulator fragment of thread t of the warp group <-> the activation tile: for half h and 8-column group j,
-// d[h][4j + {0,1}] = (row 64h + 16 (t / 32) + (t % 32) / 4, columns dcol + 8j + 2 (t % 4) + {0,1}), d[h][4j + {2,3}] = 8 rows lower.
+// The accumulator fragment of thread t of the warp group that issued the rows 64 * half .. 64 * half + 63 <-> the
+// activation tile: for 8-column group j, d[4j + {0,1}] = (row 64 half + 16 (t / 32) + (t % 32) / 4, columns
+// dcol + 8j + 2 (t % 4) + {0,1}), d[4j + {2,3}] = 8 rows lower.
 template <int N>
-__device__ __forceinline__ void acc_load(const float* act, int dcol, int t, float (&d)[2][N / 2]) {
+__device__ __forceinline__ void acc_load_half(const float* act, int dcol, int t, int half, float (&d)[N / 2]) {
+  const int r = 64 * half + 16 * (t >> 5) + ((t & 31) >> 2);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = 64 * h + 16 * (t >> 5) + ((t & 31) >> 2);
-#pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
-      const int c = dcol + 8 * j + 2 * (t & 3);
-      const float2 x = *reinterpret_cast<const float2*>(act + act_index(r, c));
-      const float2 y = *reinterpret_cast<const float2*>(act + act_index(r + 8, c));
-      d[h][4 * j] = x.x; d[h][4 * j + 1] = x.y; d[h][4 * j + 2] = y.x; d[h][4 * j + 3] = y.y;
-    }
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = dcol + 8 * j + 2 * (t & 3);
+    const float2 x = *reinterpret_cast<const float2*>(act + act_index(r, c));
+    const float2 y = *reinterpret_cast<const float2*>(act + act_index(r + 8, c));
+    d[4 * j] = x.x; d[4 * j + 1] = x.y; d[4 * j + 2] = y.x; d[4 * j + 3] = y.y;
   }
 }
 template <int N>
-__device__ __forceinline__ void acc_store(float* act, int dcol, int t, const float (&d)[2][N / 2]) {
+__device__ __forceinline__ void acc_store_half(float* act, int dcol, int t, int half, const float (&d)[N / 2]) {
+  const int r = 64 * half + 16 * (t >> 5) + ((t & 31) >> 2);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = 64 * h + 16 * (t >> 5) + ((t & 31) >> 2);
-#pragma unroll
-    for (int j = 0; j < N / 8; ++j) {
-      const int c = dcol + 8 * j + 2 * (t & 3);
-      *reinterpret_cast<float2*>(act + act_index(r, c)) = make_float2(d[h][4 * j], d[h][4 * j + 1]);
-      *reinterpret_cast<float2*>(act + act_index(r + 8, c)) = make_float2(d[h][4 * j + 2], d[h][4 * j + 3]);
-    }
+  for (int j = 0; j < N / 8; ++j) {
+    const int c = dcol + 8 * j + 2 * (t & 3);
+    *reinterpret_cast<float2*>(act + act_index(r, c)) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(act + act_index(r + 8, c)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
+}
+// both row halves issued by one warp group: d[h] is the fragment of half h
+template <int N>
+__device__ __forceinline__ void acc_store(float* act, int dcol, int t, const float (&d)[2][N / 2]) {
+  acc_store_half<N>(act, dcol, t, 0, d[0]);
+  acc_store_half<N>(act, dcol, t, 1, d[1]);
 }
 
 // 3xTF32 split
