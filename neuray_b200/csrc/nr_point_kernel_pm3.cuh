@@ -16,16 +16,21 @@
 //   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer; both warp groups meet at a
 //     256-thread barrier before a layer (its A columns come from both) and after the accumulator store.
 //   * activation tile (80 KB of shared memory, 160 columns x 128 rows, tc::act_index): hi parts at columns [0,64), lo parts
-//     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) is issued in K rounds into one accumulator at [96,160):
-//     round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only live A operand, round B
-//     (the 40 rgb_feat inputs, lo parts at [48,88)) after ray_dir_fc, then five rounds of view-pooled statistics (K 32
-//     each).  Its epilogue reads the accumulator half by half and writes base_fc.2's operand over the columns it has
+//     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) has its per-view inputs issued in two K rounds into one
+//     accumulator at [96,160): round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only
+//     live A operand, round B (the 40 rgb_feat inputs, lo parts at [48,88)) after ray_dir_fc.  Its epilogue reads the
+//     accumulator half by half, adds the point's view-pooled part and writes base_fc.2's operand over the columns it has
 //     already consumed (the same warp group owns column c and c + 32, so no other warp group reads them).
+//   * per-point layers: the view-pooled part of base_fc.0 (K 140 -> 160) and geometry_fc.0 have the same inputs for every
+//     view of a point, so they are multiplied once per point, not once per row: the pooled statistics go into a compact
+//     operand of PB rows (one per point, in tile columns [0,96) while those are dead), the eight compute warps multiply
+//     it with warp-level mma.sync (3xTF32, B read straight from the weight ring stages, warp w computes outputs
+//     8w .. 8w + 7) into a [PB][64] result in shared memory (OFF_PT), and every row of the point reads it from there.
 //   * the rest of shared memory: 4 x 16 KB weight ring (TMA bulk copies, fed by the producer group; the view-pooled
-//     base_fc.0 inputs stream through it as five more stages), the resident tile of ray_dir_fc.2, small weights, camera
-//     blocks, the row-scalar exchange, and one [32][36] transposition buffer per warp: gather (16 channels per warp group
-//     in two passes: ray_feats, then img_feats, which stay there until ray_dir_fc needs them), the cross-view pooling
-//     (pm::pool_rows) and the lane-group sums of the non-power-of-two groups all go through it.
+//     base_fc.0 weights stream through it as five more stages), the resident tile of ray_dir_fc.2, small weights, camera
+//     blocks, the row-scalar exchange, the per-point result, and one [32][36] transposition buffer per warp: gather (16
+//     channels per warp group in two passes: ray_feats, then img_feats, which stay there until ray_dir_fc needs them), the
+//     cross-view pooling (pm::pool_rows) and the lane-group sums of the non-power-of-two groups all go through it.
 #pragma once
 
 namespace pm3 {
@@ -68,7 +73,10 @@ constexpr int STG_ROW = 36;
 constexpr int STG = (NCOMP / 32) * 32 * STG_ROW;
 constexpr int OFF_XCH = OFF_STG + STG;                        // row scalars handed between the warp groups: [slot][128 rows], slots XCH_*
 constexpr int XCH_HEAD = 0, XCH_LG = 4, XCH_L2 = 5, XCH = 6 * 128;      // (o0, o1) of heads 1 and 3 | vis_fc.1 logit | vis_fc2 visibility
-constexpr int OFF_CAM = OFF_XCH + XCH;                        // que_cam [24] (padded to 32) | view_params [NR_MAX_VIEWS][20]
+constexpr int OFF_PT = OFF_XCH + XCH;                         // per-point layer outputs: [point][PT_ROW] (64 used), at most 32 points
+constexpr int PT_ROW = 72;
+constexpr int PT = 32 * PT_ROW;
+constexpr int OFF_CAM = OFF_PT + PT;                          // que_cam [24] (padded to 32) | view_params [NR_MAX_VIEWS][20]
 constexpr int CAM = 32 + NR_MAX_VIEWS * 20;
 constexpr int OFF_STAB = OFF_CAM + CAM;                       // stage_source: int4 per stage of a tile (at most 4 + 16)
 constexpr int OFF_BAR = OFF_STAB + 80;
@@ -76,7 +84,60 @@ constexpr int SMEM_FLOATS = OFF_BAR + 32;
 constexpr size_t SMEM_BYTES = size_t(SMEM_FLOATS) * 4;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 static_assert(OFF_STAB % 4 == 0, "alignment");
-static_assert((OFF_ACT * 4) % 1024 == 0 && (OFF_RD1 * 4) % 1024 == 0 && OFF_WG1 % 4 == 0 && OFF_SW % 4 == 0 && OFF_STG % 4 == 0, "alignment");
+static_assert((OFF_ACT * 4) % 1024 == 0 && (OFF_RD1 * 4) % 1024 == 0 && OFF_WG1 % 4 == 0 && OFF_SW % 4 == 0 && OFF_STG % 4 == 0 &&
+                  OFF_PT % 4 == 0, "alignment");
+// the per-point operand of a per-point layer: [point][OP_ROW] (K 160 used) in activation-tile columns [0,96), which are
+// dead while it is used (after base_fc.0's round B until its epilogue; after rgb_fc.0 until the next tile's gather)
+constexpr int OP_ROW = 164;                                   // = 4 mod 32: the 32 lanes of an A-fragment load hit 32 banks
+static_assert(32 * OP_ROW <= 3 * 4096, "per-point operand");
+
+// ---- per-point layers: [points x K] x [K x 64] on warp-level mma.sync, 3xTF32 ----
+// Compute warp w (of 8) computes outputs 8w .. 8w + 7 for all PB points of the tile: MT m16 tiles of points, and one
+// accumulator per 3xTF32 pass (hi*hi, lo*hi, hi*lo) so that the three MMAs of a K step do not wait for each other.
+template <int PB>
+struct PtAcc {
+  static constexpr int MT = (PB + 15) / 16;
+  float d[MT][3][4];
+};
+// acc += op[points][kcol + k] * W[8w + n][k], k < 8 KS: B from a weight ring stage `w` (64 rows x K32, K-major 128-byte
+// swizzle, hi slab | lo slab 2048 floats further, K steps 0 .. KS - 1).  Operand rows at or past PB read as 0.
+template <int PB, int KS>
+__device__ __forceinline__ void point_mma(PtAcc<PB>& acc, const float* __restrict__ op, int kcol, const float* __restrict__ w, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const float* __restrict__ bw = w + warp * 256 + g * 32 + t;             // tc::sw128_index(8 warp + g, 8 j + t) = bw[((2j) ^ g) << 2]
+  const float* __restrict__ aw = op + g * OP_ROW + kcol + t;
+#pragma unroll
+  for (int j = 0; j < KS; ++j) {
+    const uint32_t bh[2] = {__float_as_uint(bw[((2 * j) ^ g) << 2]), __float_as_uint(bw[((2 * j + 1) ^ g) << 2])};
+    const uint32_t bl[2] = {__float_as_uint(bw[2048 + (((2 * j) ^ g) << 2)]), __float_as_uint(bw[2048 + (((2 * j + 1) ^ g) << 2)])};
+#pragma unroll
+    for (int m = 0; m < PtAcc<PB>::MT; ++m) {
+      const bool ok0 = 16 * m + 8 <= PB || 16 * m + g < PB, ok1 = 16 * m + 16 <= PB || 16 * m + 8 + g < PB;
+      const float* __restrict__ a = aw + 16 * m * OP_ROW + 8 * j;
+      const float x[4] = {ok0 ? a[0] : 0.f, ok1 ? a[8 * OP_ROW] : 0.f, ok0 ? a[4] : 0.f, ok1 ? a[8 * OP_ROW + 4] : 0.f};
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) tc::split_tf32(x[i], ah[i], al[i]);
+      tc::mma_tf32_m16n8k8(acc.d[m][0], ah, bh);
+      tc::mma_tf32_m16n8k8(acc.d[m][1], al, bh);
+      tc::mma_tf32_m16n8k8(acc.d[m][2], ah, bl);
+    }
+  }
+}
+// the accumulated outputs -> pt[point][8w .. 8w + 7] (points < PB)
+template <int PB>
+__device__ __forceinline__ void point_store(const PtAcc<PB>& acc, float* __restrict__ pt, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int m = 0; m < PtAcc<PB>::MT; ++m) {
+    float o[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) o[i] = acc.d[m][0][i] + (acc.d[m][1][i] + acc.d[m][2][i]);
+    float* __restrict__ p = pt + (16 * m + g) * PT_ROW + 8 * warp + 2 * t;
+    if (16 * m + 8 <= PB || 16 * m + g < PB) *reinterpret_cast<float2*>(p) = make_float2(o[0], o[1]);
+    if (16 * m + 16 <= PB || 16 * m + 8 + g < PB) *reinterpret_cast<float2*>(p + 8 * PT_ROW) = make_float2(o[2], o[3]);
+  }
+}
 
 // Layer issue, executed by both compute warp groups after they wrote their A columns; warp group c multiplies rows
 // 64c .. 64c + 63.  K chunk c (of NCH) reads A columns AHI + 8c (c < NLIN) or TAILHI + 8(c - NLIN), lo parts LOOFF
@@ -322,6 +383,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   const bool idle = P2 ? false : grp >= PPW;     // a compile-time false for the power-of-two groups
   const int v = P2 ? lane % G : lane - grp * G;   // view of this row (>= rfn: padding lane)
   const int pl = P2 ? (tid & 127) / G : (warp & 3) * PPW + grp;   // point inside the block
+  const int pq = P2 ? pl : (idle ? 0 : pl);       // the same, < PB for idle lanes too: the per-point row this row reads
   const int lane0 = lane - v;                     // first lane of this point's group
   float* const stg = smem + OFF_STG + warp * 32 * STG_ROW;
   float* const xch = smem + OFF_XCH;
@@ -345,6 +407,17 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   b.wi = 0;
   b.tk = nullptr;
   const int row = b.row, wg = b.wg;
+  // a point's 16 pooled values (which every lane of the point holds) -> its row of the per-point operand: value 4q + i at
+  // column col + 8q + 4 wg + i, the layout st_own gives a row of the tile; lane v < 4 of the point stores q = v
+  auto put_point = [&](float* op, int col, const float (&st)[16]) {
+    if (v < 4 && !idle) {
+      float4 o = make_float4(st[0], st[1], st[2], st[3]);
+      if (v == 1) o = make_float4(st[4], st[5], st[6], st[7]);
+      else if (v == 2) o = make_float4(st[8], st[9], st[10], st[11]);
+      else if (v == 3) o = make_float4(st[12], st[13], st[14], st[15]);
+      *reinterpret_cast<float4*>(op + pl * OP_ROW + col + 8 * v + 4 * wg) = o;
+    }
+  };
 
   // phase stamps exist only in the DEBUG instantiation (nr_point_kernel_timing / nr_point_kernel_debug): [tile][warp group][32]
 #define PM_TICK(id)                                                                                      \
@@ -662,18 +735,23 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     }
 
     PM_TICK(6)
-    // ---------------- view pooling #1 (ibrnet.py:336-339) -> five more K rounds of base_fc.0 ----------------
-    // Every lane of a point ends a round with the point's statistics, which is exactly its row of the view-invariant
-    // operand: 8 features x (mean0, var0, mean1, var1) = K 32 per round go to A[0:32) (statistic t of feature i at column
-    // 8t + i, so warp group c pools features 4c .. 4c + 3 of the round) and are multiplied into the same accumulator, B
-    // from one ring stage per round.  The sums over the views go through the warp's transposition buffer (pool_rows); the
-    // variance comes from the weighted second moment:
+    // ---------------- view pooling #1 (ibrnet.py:336-339) -> the view-pooled part of base_fc.0, once per point ----------------
+    // Every lane of a point ends a round with the point's statistics: 8 features x (mean0, var0, mean1, var1) = K 32 per
+    // round (statistic t of feature i at column 32 R + 8t + i, so warp group c pools features 4c .. 4c + 3 of the round).
+    // They go into the point's row of the per-point operand (PB rows, K 160) and each round's K 32 is multiplied as soon
+    // as it is complete, B from the round's ring stage, into a per-point [PB][64] result that the epilogue adds to every
+    // view's row.  One barrier per round: it publishes the round's operand columns and tells thread 0 that every warp is
+    // done with the previous round's stage (the fifth stage can only load into the first one's ring slot).  The sums over
+    // the views go through the warp's transposition buffer (pool_rows); the variance comes from the weighted second moment:
     //   sum_v w (x - mu)^2 = sum_v w x^2 - mu^2 (2 - sum_v w),  mu = sum_v w x   (the reference's mean is NOT normalised)
     const float msum = gsum(mrow);
     const float w1 = mrow / (msum + 1e-8f);
     const float w0 = sigmoidf_(gate) * w1;
     {
       const float c1 = 2.f - gsum(w1), c0 = 2.f - gsum(w0);
+      float* const op = b.act;
+      const uint32_t s0 = b.wi;
+      PtAcc<PB> acc = {};
       auto round = [&](auto rc) {
         constexpr int R = decltype(rc)::value;
         float in[16], st[16];
@@ -689,19 +767,28 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
           st[4 + i] = fmaf(-st[i] * st[i], c0, st[4 + i]);
           st[12 + i] = fmaf(-st[8 + i] * st[8 + i], c1, st[12 + i]);
         }
-        st_own<4>(b, 0, 32, st);
-        issue_layer<64, 4, 0, 32, 4, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, true>(b);
+        put_point(op, 32 * R, st);
+        tc::named_sync(BAR_LAYER, NCOMP);
+        if (R > 0 && b.leader) tc::mbar_arrive(wempty + (s0 + R - 1) % NBUF);
+        tc::mbar_wait(wfull + (s0 + R) % NBUF, ((s0 + R) / NBUF) & 1);
+        point_mma<PB, 4>(acc, op, 32 * R, ring + ((s0 + R) % NBUF) * RING_STAGE, warp, lane);
       };
       round(std::integral_constant<int, 0>{}); round(std::integral_constant<int, 1>{}); round(std::integral_constant<int, 2>{});
       round(std::integral_constant<int, 3>{}); round(std::integral_constant<int, 4>{});
+      point_store(acc, smem + OFF_PT, warp, lane);
+      tc::named_sync(BAR_LAYER, NCOMP);                                            // per-point result visible; the last stage read
+      if (b.leader) tc::mbar_arrive(wempty + (s0 + 4) % NBUF);
+      b.wi += 5;
     }
 
     PM_TICK(7)
     // ---------------- base_fc on the tensor cores ----------------
+    // base_fc.0 = the per-view rounds A and B (accumulator [96,160), bias included) + the point's view-pooled part
 #pragma unroll
     for (int c0 = 0; c0 < 64; c0 += 32) {
       float x[16];
       ld_own<4>(b, 96 + c0, x);
+      add_bias_own<4>(b, x, smem + OFF_PT + pq * PT_ROW + c0);
 #pragma unroll
       for (int j = 0; j < 16; ++j) x[j] = elu(x[j]);
       st_own<4>(b, c0, 64 + c0, x);                                                // lo half 1 lands on accumulator columns already consumed
@@ -801,11 +888,13 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     const float sw2 = gsum(w2);
     const float wmean = sw2 / float(rfn);
     {
-      // two K rounds of 16 features x (mean, var) (feature i of round R at columns i and 16 + i: warp group c pools
-      // features 16R + 8q + 4c + [0,4), its xr[8R + 4q + i]) and a third with the mean weight and the constant that
-      // multiplies the bias column, one ring stage each; sums over the views through pool_rows, variance from the second
+      // geometry_fc.0, once per point: per-point operand (PB rows) = two K rounds of 16 features x (mean, var) (feature i
+      // of round R at columns 32R + i and 32R + 16 + i: warp group c pools features 16R + 8q + 4c + [0,4), its
+      // xr[8R + 4q + i]), then the mean weight and the constant that multiplies the bias column at columns 64, 65; B from
+      // three ring stages, all in the ring at once; sums over the views through pool_rows, variance from the second
       // moment (above)
       const float c2 = 2.f - sw2;
+      float* const op = b.act;
       auto ground = [&](auto rc) {
         constexpr int R = decltype(rc)::value;
         float in[16], st[16];
@@ -814,28 +903,48 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         gpool16(in, st);
 #pragma unroll
         for (int i = 0; i < 8; ++i) st[8 + i] = fmaf(-st[i] * st[i], c2, st[8 + i]);
-        st_own<4>(b, 0, 32, st);
-        issue_layer<64, 4, 0, 32, 4, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, (R > 0)>(b);
+        put_point(op, 32 * R, st);
       };
       ground(std::integral_constant<int, 0>{}); ground(std::integral_constant<int, 1>{});
-      {
-        float st[4] = {0.f, 0.f, 0.f, 0.f};
-        if (wg == 0) { st[0] = wmean; st[1] = 1.f; }
-        st_own<1>(b, 0, 32, st);
-        issue_layer<64, 1, 0, 32, 1, 0, 96, 0, 1, 0, 2048 * 4, 0, true, true, true>(b);
+      if (wg == 0 && v == 0 && !idle) {
+        *reinterpret_cast<float4*>(op + pl * OP_ROW + 64) = make_float4(wmean, 1.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(op + pl * OP_ROW + 68) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
+      tc::named_sync(BAR_LAYER, NCOMP);
+      const uint32_t s0 = b.wi;
+      PtAcc<PB> acc = {};
+#pragma unroll
+      for (int s = 0; s < 3; ++s) {
+        tc::mbar_wait(wfull + (s0 + s) % NBUF, ((s0 + s) / NBUF) & 1);
+        const float* w = ring + ((s0 + s) % NBUF) * RING_STAGE;
+        if (s < 2) point_mma<PB, 4>(acc, op, 32 * s, w, warp, lane);
+        else point_mma<PB, 1>(acc, op, 64, w, warp, lane);
+      }
+      point_store(acc, smem + OFF_PT, warp, lane);
+      tc::named_sync(BAR_LAYER, NCOMP);                                            // per-point result visible; the stages read
+      if (b.leader) {
+#pragma unroll
+        for (int s = 0; s < 3; ++s) tc::mbar_arrive(wempty + (s0 + s) % NBUF);
+      }
+      b.wi += 3;
     }
 
     PM_TICK(14)
     if (wg == 0) {
       // ---------------- geometry_fc.2 across the lanes of a point ----------------
-      // all G rows of a point hold the same 64 hidden pre-activations; lane v keeps columns [v*CPL, (v+1)*CPL)
+      // the point's 64 hidden pre-activations are its row of the per-point result; lane v takes [v*CPL, (v+1)*CPL)
       // (GE = the lanes of the point that take part: all G of a power-of-two group, else the first 8 / 4)
       const int vg = (P2 || v < GE) ? v : 0;
       float hh[CPL];
-      if constexpr (CPL >= 4) ld_row<CPL / 4>(b, 96 + vg * CPL, hh);
-      else {
-        const float2 t = *reinterpret_cast<const float2*>(b.act + tc::act_index(row, 96 + vg * CPL));
+      const float* __restrict__ hp = smem + OFF_PT + pq * PT_ROW + vg * CPL;
+      if constexpr (CPL >= 4) {
+#pragma unroll
+        for (int q = 0; q < CPL / 4; ++q) {
+          const float4 t = *reinterpret_cast<const float4*>(hp + 4 * q);
+          hh[4 * q] = t.x; hh[4 * q + 1] = t.y; hh[4 * q + 2] = t.z; hh[4 * q + 3] = t.w;
+        }
+      } else {
+        const float2 t = *reinterpret_cast<const float2*>(hp);
         hh[0] = t.x; hh[1] = t.y;
       }
 #pragma unroll
