@@ -10,7 +10,8 @@
 //     group multiplies them with wgmma and writes D back into the tile for the bias / activation epilogue, whose result
 //     goes back into the tile as the next A; warp group c issues the MMAs of rows 64c .. 64c + 63
 //   * weights stream through a 4 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk); full/empty
-//     mbarriers, the "empty" arrival comes from thread 0 once both warp groups' consuming wgmma have completed
+//     mbarriers, the "empty" barrier takes one arrival from thread 0 of each compute warp group once that warp group's
+//     consuming wgmma have completed
 #include <type_traits>
 
 #include "nr_common.cuh"
@@ -70,18 +71,9 @@ struct Blk {
   uint64_t *wfull, *wempty;     // arrays [NBUF]
   uint32_t ring_addr;           // shared-space byte address of the ring
   uint32_t wi;                  // weight stages consumed so far (same sequence in every thread)
-  bool leader;                  // thread 0: releases the ring stages
+  bool leader;                  // thread 0 of the warp group: releases the ring stages for it
   long long* tk;                // diagnostics: where run_layer drops clock64() stamps (nullptr: off)
 };
-
-// bias vector (shared memory, 16-byte aligned) added to 32 values with 128-bit loads
-__device__ __forceinline__ void add_bias32(float* x, const float* __restrict__ bias) {
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    const float4 t = *reinterpret_cast<const float4*>(bias + 4 * q);
-    x[4 * q] += t.x; x[4 * q + 1] += t.y; x[4 * q + 2] += t.z; x[4 * q + 3] += t.w;
-  }
-}
 
 namespace pm {
 template <int G>

@@ -9,12 +9,16 @@
 //     reads its accumulator columns and runs their epilogue; its registers hold its 16 of 32 (20 of 40) values.  The
 //     view-pooled statistics keep this split, because both pooled operands put one feature's statistics 8 or 16 columns
 //     apart.  Row scalars that are sums over a whole row are computed by one warp group from the full row in the tile, in
-//     the same order as a single row owner would, and handed over through a small shared array: dist-decoder head hd in
-//     warp group hd & 1, vis_fc.1 in warp group 1, vis_fc2.1 in warp group 0.  rgb_fc.1/.2 and the colour blend run in
-//     warp group 1 only, geometry_fc.2 in warp group 0 only.  (The training backward recomputes these values in that
-//     order; the forward has to agree with it bit for bit, or gradients that cancel analytically stop cancelling.)
+//     the same order as a single row owner would, and handed over through a small shared array: vis_fc.1 in warp group 1,
+//     vis_fc2.1 in warp group 0.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0
+//     only.  (The training backward recomputes these values in that order; the forward has to agree with it bit for bit,
+//     or gradients that cancel analytically stop cancelling.)
 //   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer; both warp groups meet at a
-//     256-thread barrier before a layer (its A columns come from both) and after the accumulator store.
+//     256-thread barrier before a layer (its A columns come from both) and after the accumulator store.  The dist-decoder
+//     heads are the exception (run_head): nothing in a head is pooled or needs the row-owner layout, so each warp group
+//     runs every head for its own 64 rows in the accumulator fragment (L1's A from registers, the (o0, o1) sums over the
+//     4 lanes that hold a row) and hands the outputs to warp group 0's row owners through the shared array.  The ring's
+//     "empty" barriers count one arrival per compute warp group, so each releases a head's stage on its own.
 //   * activation tile (80 KB of shared memory, 160 columns x 128 rows, tc::act_index): hi parts at columns [0,64), lo parts
 //     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) has its per-view inputs issued in two K rounds into one
 //     accumulator at [96,160): round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only
@@ -56,8 +60,7 @@ constexpr int NTHR = NCOMP + 128;                             // + a producer wa
 // compute groups take them: 128 x 24 + 256 x 240 = 64512 of the SM's 65536
 constexpr int REG_PROD = 24, REG_COMP = 240;
 static_assert(128 * REG_PROD + NCOMP * REG_COMP <= 65536, "register file");
-constexpr int BAR_LAYER = 1;                                  // named barriers of the compute warp groups: around every layer
-constexpr int BAR_XCH = 2;                                    //   warp group 1's head outputs -> warp group 0
+constexpr int BAR_LAYER = 1;                                  // named barrier of the compute warp groups: around every layer
 constexpr int TCOLS = 160;                                    // activation-tile columns
 constexpr int ACT = (TCOLS / 32) * 4096;                      // floats per activation tile
 
@@ -72,7 +75,7 @@ constexpr int OFF_STG = OFF_SW + SW;                          // gather transpos
 constexpr int STG_ROW = 36;
 constexpr int STG = (NCOMP / 32) * 32 * STG_ROW;
 constexpr int OFF_XCH = OFF_STG + STG;                        // row scalars handed between the warp groups: [slot][128 rows], slots XCH_*
-constexpr int XCH_HEAD = 0, XCH_LG = 4, XCH_L2 = 5, XCH = 6 * 128;      // (o0, o1) of heads 1 and 3 | vis_fc.1 logit | vis_fc2 visibility
+constexpr int XCH_HEAD = 0, XCH_LG = 8, XCH_L2 = 9, XCH = 10 * 128;     // (o0, o1) of the 4 heads | vis_fc.1 logit | vis_fc2 visibility
 constexpr int OFF_PT = OFF_XCH + XCH;                         // per-point layer outputs: [point][PT_ROW] (64 used), at most 32 points
 constexpr int PT_ROW = 72;
 constexpr int PT = 32 * PT_ROW;
@@ -241,6 +244,100 @@ __device__ __forceinline__ void run_layer(Blk& b) {
   issue_layer<N, NCH, AHI, 64, NLIN, TAILHI, 128, 0, 1, OFF_HI, OFF_LO, SLAB, WAIT_FULL, RELEASE, false>(b);
 }
 
+// One dist-decoder head (two K 32, N 32 layers and the (o0, o1) outputs) for the 64 rows whose MMAs this warp group
+// issues, without leaving its registers and without meeting the other warp group: L0 reads A[0:32] from the tile (both
+// warp groups wrote it before the barrier in front of the heads), its epilogue runs on the accumulator fragment, L1 takes
+// A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  This thread holds columns
+// 8j + 2q + {0, 1} of fragment rows fr and fr + 8 (q = t % 4, tc::acc_load_half); L1's A fragment wants columns 8j + q
+// and 8j + q + 4 of the same rows, which two shuffles per row and K step bring over from the quad.  Releases the head's
+// ring stage on its own (wempty counts one arrival per compute warp group).
+__device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, float* __restrict__ xo, int fr) {
+  const int lane = b.row & 31, q = lane & 3;
+  const uint32_t st = b.wi % NBUF;
+  tc::mbar_wait(b.wfull + st, (b.wi / NBUF) & 1);
+  const uint32_t base = b.ring_addr + st * (RING_STAGE * 4);
+  // L0: B hi / lo at stage floats 0 / 1024
+  float d[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) d[j] = 0.f;
+  {
+    const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + 1024 * 4);
+    tc::wgmma_fence_operand(d);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) tc::wgmma_tf32<32>(d, tc::act_desc(b.act_addr, 8 * c + (ps == 1 ? 64 : 0), b.wg), (ps == 2 ? dlo : dhi) + 2 * c);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
+    tc::wgmma_fence_operand(d);
+  }
+  // bias + ELU, then each 8-column group into L1's A layout: lane q of a quad reads lane s = 2 (q & 1) + (q >> 1) in the
+  // first shuffle and lane s ^ 2 in the second; a lane offers column 2q + (q >> 1) in the first and its other column in
+  // the second, and what arrives is column q and q + 4 (in that order for even q, swapped for odd q)
+  uint32_t ah[4][4], al[4][4];
+  {
+    const int s1 = (lane & ~3) | ((q & 1) << 1) | (q >> 1);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 bb = *reinterpret_cast<const float2*>(hw + 8 * j + 2 * q);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float x0 = elu(d[4 * j + 2 * r] + bb.x), x1 = elu(d[4 * j + 2 * r + 1] + bb.y);
+        const float r1 = __shfl_sync(0xffffffffu, q >> 1 ? x1 : x0, s1);
+        const float r2 = __shfl_sync(0xffffffffu, q >> 1 ? x0 : x1, s1 ^ 2);
+        tc::split_tf32(q & 1 ? r2 : r1, ah[j][r], al[j][r]);              // column 8j + q of row fr + 8r
+        tc::split_tf32(q & 1 ? r1 : r2, ah[j][2 + r], al[j][2 + r]);      // column 8j + q + 4
+      }
+    }
+  }
+  // L1: B hi / lo at stage floats 2048 / 3072
+  float e[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) e[j] = 0.f;
+  {
+    const uint64_t dhi = tc::smem_desc_sw128(base + 2048 * 4), dlo = tc::smem_desc_sw128(base + 3072 * 4);
+    tc::wgmma_fence_operand(e);
+    tc::wgmma_fence_operand(ah);
+    tc::wgmma_fence_operand(al);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) tc::wgmma_tf32_ra<32>(e, ps == 1 ? al[c] : ah[c], (ps == 2 ? dlo : dhi) + 2 * c);
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
+    tc::wgmma_fence_operand(e);
+    tc::wgmma_fence_operand(ah);
+    tc::wgmma_fence_operand(al);
+  }
+  if (b.leader) tc::mbar_arrive(b.wempty + st);
+  b.wi += 1;
+  // (o0, o1) of rows fr, fr + 8: this thread's 8 columns, then the quad's sum; lane q stores output q & 1 of row fr + 8 (q >> 1)
+  float p[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int c = 8 * j + 2 * q;
+    const float2 bb = *reinterpret_cast<const float2*>(hw + 32 + c);
+    const float2 wa = *reinterpret_cast<const float2*>(hw + 64 + c), wb = *reinterpret_cast<const float2*>(hw + 96 + c);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float h0 = elu(e[4 * j + 2 * r] + bb.x), h1 = elu(e[4 * j + 2 * r + 1] + bb.y);
+      p[2 * r] = fmaf(wa.y, h1, fmaf(wa.x, h0, p[2 * r]));
+      p[2 * r + 1] = fmaf(wb.y, h1, fmaf(wb.x, h0, p[2 * r + 1]));
+    }
+  }
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) p[i] += __shfl_xor_sync(0xffffffffu, p[i], o);
+  }
+  const float mine = q == 0 ? p[0] : q == 1 ? p[1] : q == 2 ? p[2] : p[3];
+  xo[(q & 1) * 128 + fr + 8 * (q >> 1)] = mine + hw[128 + (q & 1)];
+}
+
 // ---- this thread's columns of its row ----
 // own_index(b, c): the float index of column c + 4 wg of this row, c a multiple of 8 (= tc::act_index(row, c + 4 wg))
 __device__ __forceinline__ int own_index(const Blk& b, int c) { return (c >> 5) * 4096 + b.rbase + ((((c & 31) >> 2) ^ b.key) << 2); }
@@ -318,7 +415,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 
   // ---------------- one-time setup ----------------
   if (tid == 0) {
-    for (int i = 0; i < NBUF; ++i) { tc::mbar_init(wfull + i, 1); tc::mbar_init(wempty + i, 1); }
+    for (int i = 0; i < NBUF; ++i) { tc::mbar_init(wfull + i, 1); tc::mbar_init(wempty + i, 2); }   // empty: one arrival per compute warp group
     tc::mbar_init(res_bar, 1);
     tc::fence_mbar_init();
     tc::mbar_arrive_expect_tx(res_bar, tcl::RD1_SIZE * 4);
@@ -401,7 +498,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   b.wg = tid >> 7;
   b.rbase = (b.row >> 3) * 256 + (b.row & 7) * 32;
   b.key = (b.row & 7) ^ b.wg;
-  b.leader = tid == 0;
+  b.leader = b.row == 0;
   b.wfull = wfull; b.wempty = wempty;
   b.ring_addr = tc::smem_u32(ring);
   b.wi = 0;
@@ -584,51 +681,25 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     }
     gather16(32);                                                                  // img_feats: stay in the buffer until ray_dir_fc
     PM_TICK(3)
-    // head outputs (o0, o1): head hd is summed by warp group hd & 1 over the whole row
-    float hv[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
+    // the heads: each warp group runs them for the 64 rows whose MMAs it issues (run_head); A[0:32] comes from both
+    tc::fence_proxy_async_smem();
+    tc::named_sync(BAR_LAYER, NCOMP);
+    {
+      const int fr = 64 * wg + 16 * (row >> 5) + ((row & 31) >> 2);          // this thread's fragment rows: fr, fr + 8
 #pragma unroll 1
-    for (int hd = 0; hd < n_heads; ++hd) {
-      const float* __restrict__ hw_ = sw + SW_HEAD + hd * SW_HEAD_STRIDE;
-      run_layer<32, 4, 0, 4, 0, 0, 1024 * 4, 0, true, false>(b);              // L0: A[0:32]
-      {
-        float x[16];
-        ld_own<4>(b, 128, x);
-        add_bias_own<4>(b, x, hw_);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) x[j] = elu(x[j]);
-        st_own<4>(b, 32, 96, x);
-      }
-      run_layer<32, 4, 32, 4, 0, 2048 * 4, 3072 * 4, 0, false, true>(b);      // L1: A[32:64]
-      if ((hd & 1) == wg) {
-        float o0 = hw_[128], o1 = hw_[129];
-        float x[32];
-        ld_row<8>(b, 128, x);
-        add_bias32(x, hw_ + 32);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 wa = *reinterpret_cast<const float4*>(hw_ + 64 + 4 * q);
-          const float4 wb = *reinterpret_cast<const float4*>(hw_ + 96 + 4 * q);
-          const float a0 = elu(x[4 * q]), a1 = elu(x[4 * q + 1]), a2 = elu(x[4 * q + 2]), a3 = elu(x[4 * q + 3]);
-          o0 = fmaf(wa.w, a3, fmaf(wa.z, a2, fmaf(wa.y, a1, fmaf(wa.x, a0, o0))));
-          o1 = fmaf(wb.w, a3, fmaf(wb.z, a2, fmaf(wb.y, a1, fmaf(wb.x, a0, o1))));
-        }
-        if (hd == 0) { hv[0][0] = o0; hv[0][1] = o1; }
-        else if (hd == 1) { hv[1][0] = o0; hv[1][1] = o1; }
-        else if (hd == 2) { hv[2][0] = o0; hv[2][1] = o1; }
-        else { hv[3][0] = o0; hv[3][1] = o1; }
-      }
+      for (int hd = 0; hd < n_heads; ++hd) run_head(b, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
     }
     PM_TICK(4)
-    // heads 1 and 3 -> warp group 0, which alone needs them (hit and visibility go into its columns)
+    tc::named_sync(BAR_LAYER, NCOMP);                                              // head outputs -> the row owners
+    // hit and visibility go into warp group 0's columns
     float hit = 0.f, visib = 0.f;
-    if (wg == 1) {
+    if (wg == 0) {
+      float hv[4][2];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) xch[(XCH_HEAD + k) * 128 + row] = hv[1 + 2 * (k >> 1)][k & 1];
-      tc::named_arrive(BAR_XCH, NCOMP);
-    } else {
-      tc::named_sync(BAR_XCH, NCOMP);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) hv[1 + 2 * (k >> 1)][k & 1] = xch[(XCH_HEAD + k) * 128 + row];
+      for (int k = 0; k < 4; ++k) {
+        hv[k][0] = k < n_heads ? xch[(XCH_HEAD + 2 * k) * 128 + row] : 0.f;
+        hv[k][1] = k < n_heads ? xch[(XCH_HEAD + 2 * k + 1) * 128 + row] : 0.f;
+      }
       const float* vp = smem + OFF_CAM + 32 + (v < rfn ? v : 0) * 20;
       const float zc = fmaxf(zrow, 1e-5f);
       const float a = vp[15], bb = vp[16];
@@ -740,8 +811,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     // round (statistic t of feature i at column 32 R + 8t + i, so warp group c pools features 4c .. 4c + 3 of the round).
     // They go into the point's row of the per-point operand (PB rows, K 160) and each round's K 32 is multiplied as soon
     // as it is complete, B from the round's ring stage, into a per-point [PB][64] result that the epilogue adds to every
-    // view's row.  One barrier per round: it publishes the round's operand columns and tells thread 0 that every warp is
-    // done with the previous round's stage (the fifth stage can only load into the first one's ring slot).  The sums over
+    // view's row.  One barrier per round: it publishes the round's operand columns and tells the leaders (b.leader) that every
+    // warp is done with the previous round's stage (the fifth stage can only load into the first one's ring slot).  The sums over
     // the views go through the warp's transposition buffer (pool_rows); the variance comes from the weighted second moment:
     //   sum_v w (x - mu)^2 = sum_v w x^2 - mu^2 (2 - sum_v w),  mu = sum_v w x   (the reference's mean is NOT normalised)
     const float msum = gsum(mrow);

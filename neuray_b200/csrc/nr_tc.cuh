@@ -106,6 +106,14 @@ __device__ __forceinline__ void wgmma_fence_operand(float (&d)[M]) {
 #pragma unroll
   for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// the same for the A fragments of register-A wgmmas (wgmma_tf32_ra): they must stay put until the batch has completed
+template <int M, int K>
+__device__ __forceinline__ void wgmma_fence_operand(uint32_t (&a)[M][K]) {
+#pragma unroll
+  for (int i = 0; i < M; ++i)
+#pragma unroll
+    for (int k = 0; k < K; ++k) asm volatile("" : "+r"(a[i][k])::"memory");
+}
 
 // d[N/2] (this thread's part of a 64 x N fp32 accumulator) += A[64 x 8] * B[N x 8]^T, both operands in shared memory
 template <int N>
@@ -151,6 +159,21 @@ __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint6
       "%32, %33, p, 1, 1;\n}\n"
       : NR_WGMMA_D8(0), NR_WGMMA_D8(8), NR_WGMMA_D8(16), NR_WGMMA_D8(24)
       : "l"(a), "l"(b), "r"(1)
+      : "memory");
+}
+// d[N/2] += A[64 x 8] * B[N x 8]^T with A in registers: the mma.sync m16n8k8 A layout within each warp's 16 rows
+// (rows 16 (t / 32) .. + 15 of the warp group's 64; with g = (t % 32) / 4, q = t % 4: a = A(g, q), A(g + 8, q),
+// A(g, q + 4), A(g + 8, q + 4)), B in shared memory
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n}\n"
+      : NR_WGMMA_D8(0), NR_WGMMA_D8(8)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1)
       : "memory");
 }
 #undef NR_WGMMA_D8
