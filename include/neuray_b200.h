@@ -422,8 +422,8 @@ int nr_consistency_loss(const float* prob0, const float* prob1, int qn, int rn, 
 /* ---- diagnostics ------------------------------------------------------------------------------------------- */
 
 /* Self-test of the wgmma layer primitive the point kernel uses: D[128,n] = A[128,k] * W[n,k]^T with A in the shared-memory
- * activation tile and W in swizzled shared memory; mode 0 = one TF32 pass, 1 = 3xTF32 (fp32-accurate).  (n,k) in
- * {(32,32),(64,64),(16,64)}. */
+ * activation tile and W in swizzled shared memory; mode 0 = one TF32 pass, 1 = 3xTF32 (fp32-accurate), 2 = 3xTF32 with A
+ * from registers (n 16 or 32).  (n,k) in {(32,32),(64,64),(16,64)}. */
 int nr_tc_selftest(const float* A, const float* W, float* D, int n, int k, int mode, void* stream);
 
 #ifdef __cplusplus

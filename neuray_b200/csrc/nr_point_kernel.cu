@@ -72,7 +72,6 @@ struct Blk {
   uint32_t ring_addr;           // shared-space byte address of the ring
   uint32_t wi;                  // weight stages consumed so far (same sequence in every thread)
   bool leader;                  // thread 0 of the warp group: releases the ring stages for it
-  long long* tk;                // diagnostics: where run_layer drops clock64() stamps (nullptr: off)
 };
 
 namespace pm {

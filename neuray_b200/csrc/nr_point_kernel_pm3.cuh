@@ -8,23 +8,22 @@
 //     every 8-column group warp group c owns columns [4c, 4c + 4).  A warp group writes the hi/lo parts of its columns,
 //     reads its accumulator columns and runs their epilogue; its registers hold its 16 of 32 (20 of 40) values.  The
 //     view-pooled statistics keep this split, because both pooled operands put one feature's statistics 8 or 16 columns
-//     apart.  Row scalars that are sums over a whole row are computed by one warp group from the full row in the tile, in
-//     the same order as a single row owner would, and handed over through a small shared array: vis_fc.1 in warp group 1,
-//     vis_fc2.1 in warp group 0.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0
-//     only.  (The training backward recomputes these values in that order; the forward has to agree with it bit for bit,
-//     or gradients that cancel analytically stop cancelling.)
+//     apart.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0 only, each from the
+//     whole row in the tile.
 //   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer; both warp groups meet at a
 //     256-thread barrier before a layer (its A columns come from both) and after the accumulator store.  The dist-decoder
-//     heads are the exception (run_head): nothing in a head is pooled or needs the row-owner layout, so each warp group
-//     runs every head for its own 64 rows in the accumulator fragment (L1's A from registers, the (o0, o1) sums over the
-//     4 lanes that hold a row) and hands the outputs to warp group 0's row owners through the shared array.  The ring's
-//     "empty" barriers count one arrival per compute warp group, so each releases a head's stage on its own.
+//     heads (run_head) and the per-view tail base_fc.2 .. rgb_fc.0 (run_chain) are the exception: nothing in them is
+//     pooled or needs the row-owner layout, so each warp group runs them for its own 64 rows in the accumulator fragment
+//     (A from registers after the first layer, row sums over the 4 lanes that hold a row) and hands the results to the
+//     row owners through the tile and a small shared array (xch).  The ring's "empty" barriers count one arrival per
+//     compute warp group, so each releases those stages on its own.
 //   * activation tile (80 KB of shared memory, 160 columns x 128 rows, tc::act_index): hi parts at columns [0,64), lo parts
 //     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) has its per-view inputs issued in two K rounds into one
 //     accumulator at [96,160): round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only
 //     live A operand, round B (the 40 rgb_feat inputs, lo parts at [48,88)) after ray_dir_fc.  Its epilogue reads the
 //     accumulator half by half, adds the point's view-pooled part and writes base_fc.2's operand over the columns it has
-//     already consumed (the same warp group owns column c and c + 32, so no other warp group reads them).
+//     already consumed (the same warp group owns column c and c + 32, so no other warp group reads them).  run_chain
+//     leaves x2 at [96,128) and rgb_fc.0's pre-activations at [128,144).
 //   * per-point layers: the view-pooled part of base_fc.0 (K 140 -> 160) and geometry_fc.0 have the same inputs for every
 //     view of a point, so they are multiplied once per point, not once per row: the pooled statistics go into a compact
 //     operand of PB rows (one per point, in tile columns [0,96) while those are dead), the eight compute warps multiply
@@ -75,7 +74,8 @@ constexpr int OFF_STG = OFF_SW + SW;                          // gather transpos
 constexpr int STG_ROW = 36;
 constexpr int STG = (NCOMP / 32) * 32 * STG_ROW;
 constexpr int OFF_XCH = OFF_STG + STG;                        // row scalars handed between the warp groups: [slot][128 rows], slots XCH_*
-constexpr int XCH_HEAD = 0, XCH_LG = 8, XCH_L2 = 9, XCH = 10 * 128;     // (o0, o1) of the 4 heads | vis_fc.1 logit | vis_fc2 visibility
+// (o0, o1) of the 4 heads; once the heads' outputs are read, the chain's row scalars w1, mrow, dd[0..3] | vis_fc2 visibility
+constexpr int XCH_HEAD = 0, XCH_ROW = 0, XCH_L2 = 8, XCH = 9 * 128;
 constexpr int OFF_PT = OFF_XCH + XCH;                         // per-point layer outputs: [point][PT_ROW] (64 used), at most 32 points
 constexpr int PT_ROW = 72;
 constexpr int PT = 32 * PT_ROW;
@@ -150,18 +150,13 @@ __device__ __forceinline__ void point_store(const PtAcc<PB>& acc, float* __restr
 template <int N, int NCH, int AHI, int LOOFF, int NLIN, int TAILHI, int DCOL, int CB0, int NSTG, uint32_t OFF_HI, uint32_t OFF_LO,
           uint32_t SLAB, bool WAIT_FULL, bool RELEASE, bool ACC>
 __device__ __forceinline__ void issue_layer(Blk& b) {
-  // b.tk: diagnostics of ONE layer's round trip (debug instantiation only; a compile-time null otherwise)
-  if (b.tk) b.tk[0] = clock64();
   tc::fence_proxy_async_smem();              // this thread's A columns -> visible to the tensor cores
-  if (b.tk) b.tk[1] = clock64();
   tc::named_sync(BAR_LAYER, NCOMP);
-  if (b.tk) b.tk[2] = clock64();
   const uint32_t st0 = b.wi % NBUF;
   if (WAIT_FULL) {
 #pragma unroll
     for (int s = 0; s < NSTG; ++s) tc::mbar_wait(b.wfull + ((st0 + s) % NBUF), ((b.wi + s) / NBUF) & 1);
   }
-  if (b.tk) b.tk[3] = clock64();
   float d[N / 2];
   if (ACC) tc::acc_load_half<N>(b.act, DCOL, b.row, b.wg, d);
   else {
@@ -191,10 +186,8 @@ __device__ __forceinline__ void issue_layer(Blk& b) {
     }
   }
   tc::wgmma_commit();
-  if (b.tk) b.tk[4] = clock64();
   tc::wgmma_wait_all();
   tc::wgmma_fence_operand(d);
-  if (b.tk) b.tk[5] = clock64();
   tc::acc_store_half<N>(b.act, DCOL, b.row, b.wg, d);
   tc::named_sync(BAR_LAYER, NCOMP);          // outputs in the tile; both warp groups' reads of the stages have completed
   if (RELEASE) {
@@ -204,7 +197,6 @@ __device__ __forceinline__ void issue_layer(Blk& b) {
     }
     b.wi += NSTG;
   }
-  if (b.tk) b.tk[6] = clock64();
 }
 // Same, B operand = a resident shared-memory tile at byte address `base` (hi slabs first, SLAB bytes apart; lo parts
 // OFF_LO bytes further): no ring accounting.
@@ -244,13 +236,101 @@ __device__ __forceinline__ void run_layer(Blk& b) {
   issue_layer<N, NCH, AHI, 64, NLIN, TAILHI, 128, 0, 1, OFF_HI, OFF_LO, SLAB, WAIT_FULL, RELEASE, false>(b);
 }
 
+// ---- layers in the accumulator fragment of the warp group that issues them (the heads and the per-view chain) ----
+// This thread holds columns 8j + 2q + {0, 1} of fragment rows fr and fr + 8 (q = t % 4, tc::acc_load_half):
+// d[4j + 2r + e] is column 8j + 2q + e of row fr + 8r.  B of K step c sits at descriptor + (c >> 2) SLAB16 + 2 (c & 3)
+// of the hi (passes 0, 1) or lo (pass 2) descriptor; the passes and K steps go in issue_layer's order, so the
+// accumulators get the same products in the same order as a round trip through the tile.
+// d = A x B, A = tile columns [0, 8 KS) (hi) / [64, 64 + 8 KS) (lo) of this warp group's 64 rows.  Committed, not waited for.
+template <int KS, int SLAB16>
+__device__ __forceinline__ void issue_frag_ss(const Blk& b, float (&d)[16], uint64_t dhi, uint64_t dlo) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) d[j] = 0.f;
+  tc::wgmma_fence_operand(d);
+  tc::wgmma_fence();
+#pragma unroll
+  for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+    for (int c = 0; c < KS; ++c)
+      tc::wgmma_tf32<32>(d, tc::act_desc(b.act_addr, 8 * c + (ps == 1 ? 64 : 0), b.wg), (ps == 2 ? dlo : dhi) + (c >> 2) * SLAB16 + 2 * (c & 3));
+  }
+  tc::wgmma_commit();
+}
+// d = A x B, A from registers: K step c from ah[c] / al[c] (c < KS <= KA).  Committed, not waited for: the A registers and
+// d stay pinned until wait_frag.
+template <int N, int KS, int SLAB16, int KA>
+__device__ __forceinline__ void issue_frag_ra(float (&d)[N / 2], uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4], uint64_t dhi, uint64_t dlo) {
+#pragma unroll
+  for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
+  tc::wgmma_fence_operand(d);
+#pragma unroll
+  for (int c = 0; c < KS; ++c)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ah[c][i]), "+r"(al[c][i])::"memory");
+  tc::wgmma_fence();
+#pragma unroll
+  for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+    for (int c = 0; c < KS; ++c) tc::wgmma_tf32_ra<N>(d, ps == 1 ? al[c] : ah[c], (ps == 2 ? dlo : dhi) + (c >> 2) * SLAB16 + 2 * (c & 3));
+  }
+  tc::wgmma_commit();
+}
+template <int N, int KS, int KA>
+__device__ __forceinline__ void wait_frag_ra(float (&d)[N / 2], uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4]) {
+  tc::wgmma_wait_all();
+  tc::wgmma_fence_operand(d);
+#pragma unroll
+  for (int c = 0; c < KS; ++c)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ah[c][i]), "+r"(al[c][i])::"memory");
+}
+__device__ __forceinline__ void wait_frag(float (&d)[16]) {
+  tc::wgmma_wait_all();
+  tc::wgmma_fence_operand(d);
+}
+// An N = 32 fragment x (after its epilogue) -> the A fragments of the next layer's 4 K steps, split into hi / lo
+// (ah[j], al[j], j < 4).  A K step wants columns 8j + q and 8j + q + 4 of rows fr, fr + 8 (tc::wgmma_tf32_ra): lane q of
+// a quad reads lane s = 2 (q & 1) + (q >> 1) in the first shuffle and lane s ^ 2 in the second; a lane offers column
+// 2q + (q >> 1) in the first and its other column in the second, and what arrives is column q and q + 4 (in that order
+// for even q, swapped for odd q).
+template <int KA>
+__device__ __forceinline__ void frag_to_a(const float (&x)[16], int lane, uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4]) {
+  const int q = lane & 3, s1 = (lane & ~3) | ((q & 1) << 1) | (q >> 1);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float x0 = x[4 * j + 2 * r], x1 = x[4 * j + 2 * r + 1];
+      const float r1 = __shfl_sync(0xffffffffu, q >> 1 ? x1 : x0, s1);
+      const float r2 = __shfl_sync(0xffffffffu, q >> 1 ? x0 : x1, s1 ^ 2);
+      tc::split_tf32(q & 1 ? r2 : r1, ah[j][r], al[j][r]);              // column 8j + q of row fr + 8r
+      tc::split_tf32(q & 1 ? r1 : r2, ah[j][2 + r], al[j][2 + r]);      // column 8j + q + 4
+    }
+  }
+}
+// s[r] = bias + sum_c w[c] z(row fr + 8r, column c) over the 32 columns of an N = 32 fragment z, one fmaf per column in
+// column order (the order the training recompute and a single row owner use), in every lane of the quad: column
+// 8j + 2q' + e comes over from lane q' of the quad
+__device__ __forceinline__ void row_dot(const float (&z)[16], const float* __restrict__ w, float bias, int lane, float (&s)[2]) {
+  s[0] = s[1] = bias;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+#pragma unroll
+    for (int qs = 0; qs < 4; ++qs) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) s[r] = fmaf(w[8 * j + 2 * qs + e], __shfl_sync(0xffffffffu, z[4 * j + 2 * r + e], (lane & ~3) | qs), s[r]);
+      }
+    }
+  }
+}
+
 // One dist-decoder head (two K 32, N 32 layers and the (o0, o1) outputs) for the 64 rows whose MMAs this warp group
 // issues, without leaving its registers and without meeting the other warp group: L0 reads A[0:32] from the tile (both
 // warp groups wrote it before the barrier in front of the heads), its epilogue runs on the accumulator fragment, L1 takes
-// A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  This thread holds columns
-// 8j + 2q + {0, 1} of fragment rows fr and fr + 8 (q = t % 4, tc::acc_load_half); L1's A fragment wants columns 8j + q
-// and 8j + q + 4 of the same rows, which two shuffles per row and K step bring over from the quad.  Releases the head's
-// ring stage on its own (wempty counts one arrival per compute warp group).
+// A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  Releases the head's ring stage on its own
+// (wempty counts one arrival per compute warp group).
 __device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, float* __restrict__ xo, int fr) {
   const int lane = b.row & 31, q = lane & 3;
   const uint32_t st = b.wi % NBUF;
@@ -258,61 +338,24 @@ __device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, f
   const uint32_t base = b.ring_addr + st * (RING_STAGE * 4);
   // L0: B hi / lo at stage floats 0 / 1024
   float d[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) d[j] = 0.f;
-  {
-    const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + 1024 * 4);
-    tc::wgmma_fence_operand(d);
-    tc::wgmma_fence();
-#pragma unroll
-    for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-      for (int c = 0; c < 4; ++c) tc::wgmma_tf32<32>(d, tc::act_desc(b.act_addr, 8 * c + (ps == 1 ? 64 : 0), b.wg), (ps == 2 ? dlo : dhi) + 2 * c);
-    }
-    tc::wgmma_commit();
-    tc::wgmma_wait_all();
-    tc::wgmma_fence_operand(d);
-  }
-  // bias + ELU, then each 8-column group into L1's A layout: lane q of a quad reads lane s = 2 (q & 1) + (q >> 1) in the
-  // first shuffle and lane s ^ 2 in the second; a lane offers column 2q + (q >> 1) in the first and its other column in
-  // the second, and what arrives is column q and q + 4 (in that order for even q, swapped for odd q)
+  issue_frag_ss<4, 0>(b, d, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
+  wait_frag(d);
+  // bias + ELU, then into L1's A layout
   uint32_t ah[4][4], al[4][4];
-  {
-    const int s1 = (lane & ~3) | ((q & 1) << 1) | (q >> 1);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 bb = *reinterpret_cast<const float2*>(hw + 8 * j + 2 * q);
+  for (int j = 0; j < 4; ++j) {
+    const float2 bb = *reinterpret_cast<const float2*>(hw + 8 * j + 2 * q);
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const float x0 = elu(d[4 * j + 2 * r] + bb.x), x1 = elu(d[4 * j + 2 * r + 1] + bb.y);
-        const float r1 = __shfl_sync(0xffffffffu, q >> 1 ? x1 : x0, s1);
-        const float r2 = __shfl_sync(0xffffffffu, q >> 1 ? x0 : x1, s1 ^ 2);
-        tc::split_tf32(q & 1 ? r2 : r1, ah[j][r], al[j][r]);              // column 8j + q of row fr + 8r
-        tc::split_tf32(q & 1 ? r1 : r2, ah[j][2 + r], al[j][2 + r]);      // column 8j + q + 4
-      }
+    for (int r = 0; r < 2; ++r) {
+      d[4 * j + 2 * r] = elu(d[4 * j + 2 * r] + bb.x);
+      d[4 * j + 2 * r + 1] = elu(d[4 * j + 2 * r + 1] + bb.y);
     }
   }
+  frag_to_a(d, lane, ah, al);
   // L1: B hi / lo at stage floats 2048 / 3072
   float e[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) e[j] = 0.f;
-  {
-    const uint64_t dhi = tc::smem_desc_sw128(base + 2048 * 4), dlo = tc::smem_desc_sw128(base + 3072 * 4);
-    tc::wgmma_fence_operand(e);
-    tc::wgmma_fence_operand(ah);
-    tc::wgmma_fence_operand(al);
-    tc::wgmma_fence();
-#pragma unroll
-    for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-      for (int c = 0; c < 4; ++c) tc::wgmma_tf32_ra<32>(e, ps == 1 ? al[c] : ah[c], (ps == 2 ? dlo : dhi) + 2 * c);
-    }
-    tc::wgmma_commit();
-    tc::wgmma_wait_all();
-    tc::wgmma_fence_operand(e);
-    tc::wgmma_fence_operand(ah);
-    tc::wgmma_fence_operand(al);
-  }
+  issue_frag_ra<32, 4, 0>(e, ah, al, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
+  wait_frag_ra<32, 4>(e, ah, al);
   if (b.leader) tc::mbar_arrive(b.wempty + st);
   b.wi += 1;
   // (o0, o1) of rows fr, fr + 8: this thread's 8 columns, then the quad's sum; lane q stores output q & 1 of row fr + 8 (q >> 1)
@@ -336,6 +379,131 @@ __device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, f
   }
   const float mine = q == 0 ? p[0] : q == 1 ? p[1] : q == 2 ? p[2] : p[3];
   xo[(q & 1) * 128 + fr + 8 * (q >> 1)] = mine + hw[128 + (q & 1)];
+}
+
+// The per-view tail base_fc.2 -> vis_fc.0 -> vis_fc.2 -> vis_fc2.0 -> rgb_fc.0 for the 64 rows whose MMAs this warp
+// group issues, in its accumulator fragment and without meeting the other warp group: nothing in it pools across views.
+// base_fc.2 reads its A (K 64) from the tile, where both warp groups' row owners wrote it before the barrier in front of
+// the chain, together with the row scalars w1, mrow and dd[0..3] in xch slots XCH_ROW + [0,6); every later layer takes
+// A from registers.  vis_fc.1 and vis_fc2.1 are summed by the quad that holds a row, in column order (row_dot), so every
+// value is bit-identical to a round trip through the row owners.  Leaves x2 (base_fc.2's output +
+// the vis_fc residual) in tile columns [96,128), rgb_fc.0's pre-activations in [128,144) and vis2 in xch slot XCH_L2.
+// Ring stages (each warp group waits and releases on its own): base_fc.2 | vis_fc.0 (B hi / lo at stage floats
+// 0 / 1024) + vis_fc.2 (2048 / 3072) | vis_fc2.0 (0 / 1024) + rgb_fc.0 (2048 / 3072, K step 4 512 floats further).
+// tk: where the phase stamps after base_fc.2, vis_fc.0, vis_fc.2 and vis_fc2.0 go (nullptr: none).
+__device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, float* __restrict__ xch, int fr, long long* tk) {
+  const int lane = b.row & 31, q = lane & 3;
+  auto stage = [&](int s) {
+    const uint32_t i = b.wi + s;
+    tc::mbar_wait(b.wfull + i % NBUF, (i / NBUF) & 1);
+    return b.ring_addr + (i % NBUF) * (RING_STAGE * 4);
+  };
+  auto release = [&](int s) {
+    if (b.leader) tc::mbar_arrive(b.wempty + (b.wi + s) % NBUF);
+  };
+  // base_fc.2: K = 64 from the tile; the row scalars load under its MMAs
+  uint32_t base = stage(0);
+  float d[16];
+  issue_frag_ss<8, 256>(b, d, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 2048 * 4));
+  float w1[2], mr[2], t0[2], t1[2];                 // t0, t1: rgb_fc.0's K tail, columns 32 + q and 36 + q (t0 of lane 0 is vis2)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float* __restrict__ x = xch + XCH_ROW * 128 + fr + 8 * r;
+    w1[r] = x[0];
+    mr[r] = x[128];
+    t0[r] = q == 0 ? 0.f : x[(1 + q) * 128];
+    t1[r] = q == 0 ? x[5 * 128] : 0.f;
+  }
+  wait_frag(d);
+  release(0);
+  float xr[16];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 bb = *reinterpret_cast<const float2*>(sw + SW_B1B + 8 * j + 2 * q);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      xr[4 * j + 2 * r] = elu(d[4 * j + 2 * r] + bb.x);
+      xr[4 * j + 2 * r + 1] = elu(d[4 * j + 2 * r + 1] + bb.y);
+    }
+  }
+  uint32_t ah[4][4], al[4][4];
+  frag_to_a(xr, lane, ah, al);
+  if (tk) tk[0] = clock64();
+  // vis_fc.0 (row scale w1 in the epilogue)
+  base = stage(1);
+  issue_frag_ra<32, 4, 0>(d, ah, al, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
+  wait_frag_ra<32, 4>(d, ah, al);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 bb = *reinterpret_cast<const float2*>(sw + SW_V0B + 8 * j + 2 * q);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      d[4 * j + 2 * r] = elu(fmaf(w1[r], d[4 * j + 2 * r], bb.x));
+      d[4 * j + 2 * r + 1] = elu(fmaf(w1[r], d[4 * j + 2 * r + 1], bb.y));
+    }
+  }
+  frag_to_a(d, lane, ah, al);
+  if (tk) tk[1] = clock64();
+  // vis_fc.2, then vis_fc.1 (the vis_fc.0 outputs' dot product; under the MMAs, with their A registers pinned, it spills)
+  float e[16];
+  issue_frag_ra<32, 4, 0>(e, ah, al, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
+  wait_frag_ra<32, 4>(e, ah, al);
+  release(1);
+  float visa[2];
+  {
+    float lg[2];
+    row_dot(d, sw + SW_V1LW, sw[SW_V1LB], lane, lg);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) visa[r] = sigmoidf_(elu(lg[r])) * mr[r];
+  }
+  // x2 = xr + vis_fc.2's outputs: A of vis_fc2.0 and of rgb_fc.0's first 4 K steps
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 bb = *reinterpret_cast<const float2*>(sw + SW_V1B + 8 * j + 2 * q);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      xr[4 * j + 2 * r] += elu(e[4 * j + 2 * r] + bb.x);
+      xr[4 * j + 2 * r + 1] += elu(e[4 * j + 2 * r + 1] + bb.y);
+    }
+  }
+  uint32_t a2h[5][4], a2l[5][4];
+  frag_to_a(xr, lane, a2h, a2l);
+  if (tk) tk[2] = clock64();
+  // vis_fc2.0; x2 goes to the tile under its MMAs
+  base = stage(2);
+  issue_frag_ra<32, 4, 0>(d, a2h, a2l, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
+  tc::acc_store_half<32>(b.act, 96, b.row, b.wg, xr);
+  wait_frag_ra<32, 4>(d, a2h, a2l);
+  float vis2[2];
+  {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 bb = *reinterpret_cast<const float2*>(sw + SW_V20B + 8 * j + 2 * q);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        d[4 * j + 2 * r] = elu(fmaf(visa[r], d[4 * j + 2 * r], bb.x));
+        d[4 * j + 2 * r + 1] = elu(fmaf(visa[r], d[4 * j + 2 * r + 1], bb.y));
+      }
+    }
+    float l2[2];
+    row_dot(d, sw + SW_V21W, sw[SW_V21B], lane, l2);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) vis2[r] = sigmoidf_(l2[r]) * mr[r];
+  }
+  if (tk) tk[3] = clock64();
+  // rgb_fc.0: K = 32 (x2) + the tail (vis2, dd0, dd1, dd2 | dd3, 0, 0, 0), N = 16
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    tc::split_tf32(q == 0 ? vis2[r] : t0[r], a2h[4][r], a2l[4][r]);
+    tc::split_tf32(t1[r], a2h[4][2 + r], a2l[4][2 + r]);
+  }
+  float g[8];
+  issue_frag_ra<16, 5, 128>(g, a2h, a2l, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
+  if (q < 2) xch[XCH_L2 * 128 + fr + 8 * q] = q ? vis2[1] : vis2[0];
+  wait_frag_ra<16, 5>(g, a2h, a2l);
+  release(2);
+  b.wi += 3;
+  tc::acc_store_half<16>(b.act, 128, b.row, b.wg, g);
 }
 
 // ---- this thread's columns of its row ----
@@ -502,8 +670,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   b.wfull = wfull; b.wempty = wempty;
   b.ring_addr = tc::smem_u32(ring);
   b.wi = 0;
-  b.tk = nullptr;
   const int row = b.row, wg = b.wg;
+  const int fr = 64 * wg + 16 * (row >> 5) + ((row & 31) >> 2);           // this thread's accumulator fragment rows: fr, fr + 8
   // a point's 16 pooled values (which every lane of the point holds) -> its row of the per-point operand: value 4q + i at
   // column col + 8q + 4 wg + i, the layout st_own gives a row of the tile; lane v < 4 of the point stores q = v
   auto put_point = [&](float* op, int col, const float (&st)[16]) {
@@ -684,11 +852,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     // the heads: each warp group runs them for the 64 rows whose MMAs it issues (run_head); A[0:32] comes from both
     tc::fence_proxy_async_smem();
     tc::named_sync(BAR_LAYER, NCOMP);
-    {
-      const int fr = 64 * wg + 16 * (row >> 5) + ((row & 31) >> 2);          // this thread's fragment rows: fr, fr + 8
 #pragma unroll 1
-      for (int hd = 0; hd < n_heads; ++hd) run_head(b, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
-    }
+    for (int hd = 0; hd < n_heads; ++hd) run_head(b, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
     PM_TICK(4)
     tc::named_sync(BAR_LAYER, NCOMP);                                              // head outputs -> the row owners
     // hit and visibility go into warp group 0's columns
@@ -864,93 +1029,30 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       for (int j = 0; j < 16; ++j) x[j] = elu(x[j]);
       st_own<4>(b, c0, 64 + c0, x);                                                // lo half 1 lands on accumulator columns already consumed
     }
+    {
+      // the row scalars of the chain's fragment rows, into the heads' exchange slots (dead since the heads' outputs were
+      // read): w1, mrow, dd[0] from warp group 0, dd[1..3] from warp group 1
+      const float rs[6] = {w1, mrow, dd[0], dd[1], dd[2], dd[3]};
+#pragma unroll
+      for (int k = 0; k < 3; ++k) xch[(XCH_ROW + 3 * wg + k) * 128 + row] = wg ? rs[3 + k] : rs[k];
+    }
     PM_TICK(8)
-    run_layer<32, 8, 0, 8, 0, 0, 2048 * 4, 4096, true, true>(b);                  // base_fc.2: K = 64
+    // ---------------- base_fc.2, vis_fc, vis_fc2, rgb_fc.0: each warp group for its own 64 rows (run_chain) ----------------
+    tc::fence_proxy_async_smem();
+    tc::named_sync(BAR_LAYER, NCOMP);
+    {
+      long long* tk = nullptr;                                                     // phase stamps 9 .. 12 inside the chain
+      if constexpr (DEBUG) {
+        if (kp.timing != nullptr && blockIdx.x == 0 && row == 0 && it < 64) tk = kp.timing + (it * 2 + wg) * 32 + 9;
+      }
+      run_chain(b, sw, xch, fr, tk);
+    }
+    tc::named_sync(BAR_LAYER, NCOMP);                                              // x2, rgb_fc.0 and vis2 -> the row owners
     float xr[16];
-    ld_own<4>(b, 128, xr);
-    add_bias_own<4>(b, xr, sw + SW_B1B);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) xr[j] = elu(xr[j]);
-    st_own<4>(b, 0, 64, xr);
-
-    PM_TICK(9)
-    // ---------------- vis_fc, vis_fc2, rgb_fc ----------------
-    if constexpr (DEBUG) {
-      if (kp.timing != nullptr && blockIdx.x == 0 && row == 0 && it < 64) b.tk = kp.timing + (it * 2 + wg) * 32 + 16;
-    }
-    run_layer<32, 4, 0, 4, 0, 0, 1024 * 4, 0, true, false>(b);                     // vis_fc.0 (row scale folded into the epilogue)
-    {
-      float x[16];
-      ld_own<4>(b, 128, x);
-      if (b.tk) b.tk[7] = clock64();
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 bb = own4(b, sw + SW_V0B, q);
-        x[4 * q] = elu(fmaf(w1, x[4 * q], bb.x)); x[4 * q + 1] = elu(fmaf(w1, x[4 * q + 1], bb.y));
-        x[4 * q + 2] = elu(fmaf(w1, x[4 * q + 2], bb.z)); x[4 * q + 3] = elu(fmaf(w1, x[4 * q + 3], bb.w));
-      }
-      if (wg == 1) {                                                               // vis_fc.1 over the whole row; read after vis_fc.2's barrier
-        float lg = sw[SW_V1LB];
-        float y[32];
-        ld_row<8>(b, 128, y);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 bb = *reinterpret_cast<const float4*>(sw + SW_V0B + 4 * q);
-          const float4 wl = *reinterpret_cast<const float4*>(sw + SW_V1LW + 4 * q);
-          y[4 * q] = elu(fmaf(w1, y[4 * q], bb.x)); y[4 * q + 1] = elu(fmaf(w1, y[4 * q + 1], bb.y));
-          y[4 * q + 2] = elu(fmaf(w1, y[4 * q + 2], bb.z)); y[4 * q + 3] = elu(fmaf(w1, y[4 * q + 3], bb.w));
-          lg = fmaf(wl.w, y[4 * q + 3], fmaf(wl.z, y[4 * q + 2], fmaf(wl.y, y[4 * q + 1], fmaf(wl.x, y[4 * q], lg))));
-        }
-        xch[XCH_LG * 128 + row] = lg;
-      }
-      if (b.tk) b.tk[8] = clock64();
-      st_own<4>(b, 32, 96, x);
-      if (b.tk) { b.tk[9] = clock64(); b.tk = nullptr; }
-    }
-    PM_TICK(10)
-    run_layer<32, 4, 32, 4, 0, 2048 * 4, 3072 * 4, 0, false, true>(b);             // vis_fc.2 outputs 0..31 (residual)
-    const float visa = sigmoidf_(elu(xch[XCH_LG * 128 + row])) * mrow;
-    {
-      float x[16];
-      ld_own<4>(b, 128, x);
-      add_bias_own<4>(b, x, sw + SW_V1B);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) xr[j] += elu(x[j]);
-      st_own<4>(b, 0, 64, xr);
-    }
-    PM_TICK(11)
-    run_layer<32, 4, 0, 4, 0, 0, 1024 * 4, 0, true, false>(b);                     // vis_fc2.0
-    float vis2 = 0.f;
-    {
-      // vis_fc2.1 over the whole row in warp group 0, which needs it now: A[32:40] = vis, ray_diff, 0; warp group 1 reads
-      // it after rgb_fc.0's barrier
-      float y[4];
-      if (wg == 0) {
-        float l2 = sw[SW_V21B];
-        float x[32];
-        ld_row<8>(b, 128, x);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 bb = *reinterpret_cast<const float4*>(sw + SW_V20B + 4 * q);
-          const float4 wl = *reinterpret_cast<const float4*>(sw + SW_V21W + 4 * q);
-          l2 = fmaf(wl.x, elu(fmaf(visa, x[4 * q], bb.x)), l2); l2 = fmaf(wl.y, elu(fmaf(visa, x[4 * q + 1], bb.y)), l2);
-          l2 = fmaf(wl.z, elu(fmaf(visa, x[4 * q + 2], bb.z)), l2); l2 = fmaf(wl.w, elu(fmaf(visa, x[4 * q + 3], bb.w)), l2);
-        }
-        vis2 = sigmoidf_(l2) * mrow;
-        xch[XCH_L2 * 128 + row] = vis2;
-        y[0] = vis2; y[1] = dd[0]; y[2] = dd[1]; y[3] = dd[2];
-      } else {
-        y[0] = dd[3]; y[1] = 0.f; y[2] = 0.f; y[3] = 0.f;
-      }
-      st_own<1>(b, 32, 96, y);
-    }
-    PM_TICK(12)
-    run_layer<16, 5, 0, 4, 32, 2048 * 4, 3072 * 4, 2048, false, true>(b);          // rgb_fc.0: K = 32 + 8, N = 16
+    ld_own<4>(b, 96, xr);
+    const float vis2 = xch[XCH_L2 * 128 + row];
     float xg[16];                                                                  // warp group 1: rgb_fc.0 outputs, for the colour blend at the end
-    if (wg == 1) {
-      vis2 = xch[XCH_L2 * 128 + row];
-      ld_row<4>(b, 128, xg);
-    }
+    if (wg == 1) ld_row<4>(b, 128, xg);
 
     PM_TICK(13)
     // ---------------- view pooling #2 (ibrnet.py:352-353) -> geometry_fc.0 on the tensor cores ----------------

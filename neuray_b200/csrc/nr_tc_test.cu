@@ -1,15 +1,17 @@
 // Self-test of the wgmma layer primitive in nr_tc.cuh: D[128 x N] = A[128 x K] * W[N x K]^T with A in the shared-memory
 // activation tile, W in shared memory (K-major, 128B swizzle), fp32 accumulators in registers written back into the tile.
-// mode 0: single TF32 pass (PASSES = 1), mode 1: 3xTF32 (PASSES = 3).  tests/test_tc_gpu.py compares against an fp64 reference.
+// mode 0: single TF32 pass, mode 1: 3xTF32, mode 2: 3xTF32 with A from registers (tc::wgmma_tf32_ra, N = 16 and 32).
+// tests/test_tc_gpu.py and tests/test_tc_ra_gpu.py compare against an fp64 reference.
 #include "nr_common.cuh"
 #include "nr_tc.cuh"
 
 namespace nr {
 
-template <int N, int K, int PASSES>
+template <int N, int K, int MODE>
 __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ W,
                                                            float* __restrict__ D) {
   static_assert(K % 32 == 0 && N % 16 == 0, "shape");
+  constexpr int PASSES = MODE == 0 ? 1 : 3;
   constexpr int KS = K / 32;                       // 32-wide K slabs of the B tile
   constexpr int SLAB = N * 32;                     // floats per slab
   constexpr int COLS = 2 * K + 64;                 // activation tile: A_hi K | A_lo K | D N (<= 64)
@@ -51,20 +53,50 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
       for (int j = 0; j < N / 2; ++j) d[h][j] = 0.f;
     tc::wgmma_fence_operand(d[0]);
     tc::wgmma_fence_operand(d[1]);
-    tc::wgmma_fence();
+    if constexpr (MODE == 2) {
+      // A fragments straight from global memory: row 64 h + 16 (tid / 32) + g (+ 8), column 8 s + q (+ 4) of half h, K step s
+      const int g = (tid & 31) >> 2, q = tid & 3;
+      uint32_t ah[2][K / 8][4], al[2][K / 8][4];
 #pragma unroll
-    for (int ps = 0; ps < PASSES; ++ps) {
-      const int a_c = (ps == 1) ? cA_lo : cA_hi;
-      const float* b_s = (ps == 2) ? sBlo : sBhi;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int s = 0; s < K / 8; ++s) {
-        const uint64_t bd = tc::smem_desc_sw128(tc::smem_u32(b_s + (s >> 2) * SLAB) + (s & 3) * 32);
-        tc::wgmma_tf32<N>(d[0], tc::act_desc(sa, a_c + 8 * s, 0), bd);
-        tc::wgmma_tf32<N>(d[1], tc::act_desc(sa, a_c + 8 * s, 1), bd);
+        for (int s = 0; s < K / 8; ++s)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            tc::split_tf32(A[size_t(64 * h + 16 * (tid >> 5) + g + 8 * (i & 1)) * K + 8 * s + q + 4 * (i >> 1)], ah[h][s][i], al[h][s][i]);
+      tc::wgmma_fence_operand(ah[0]); tc::wgmma_fence_operand(ah[1]);
+      tc::wgmma_fence_operand(al[0]); tc::wgmma_fence_operand(al[1]);
+      tc::wgmma_fence();
+#pragma unroll
+      for (int ps = 0; ps < 3; ++ps) {
+        const float* b_s = (ps == 2) ? sBlo : sBhi;
+#pragma unroll
+        for (int s = 0; s < K / 8; ++s) {
+          const uint64_t bd = tc::smem_desc_sw128(tc::smem_u32(b_s + (s >> 2) * SLAB) + (s & 3) * 32);
+          tc::wgmma_tf32_ra<N>(d[0], ps == 1 ? al[0][s] : ah[0][s], bd);
+          tc::wgmma_tf32_ra<N>(d[1], ps == 1 ? al[1][s] : ah[1][s], bd);
+        }
       }
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
+      tc::wgmma_fence_operand(ah[0]); tc::wgmma_fence_operand(ah[1]);
+      tc::wgmma_fence_operand(al[0]); tc::wgmma_fence_operand(al[1]);
+    } else {
+      tc::wgmma_fence();
+#pragma unroll
+      for (int ps = 0; ps < PASSES; ++ps) {
+        const int a_c = (ps == 1) ? cA_lo : cA_hi;
+        const float* b_s = (ps == 2) ? sBlo : sBhi;
+#pragma unroll
+        for (int s = 0; s < K / 8; ++s) {
+          const uint64_t bd = tc::smem_desc_sw128(tc::smem_u32(b_s + (s >> 2) * SLAB) + (s & 3) * 32);
+          tc::wgmma_tf32<N>(d[0], tc::act_desc(sa, a_c + 8 * s, 0), bd);
+          tc::wgmma_tf32<N>(d[1], tc::act_desc(sa, a_c + 8 * s, 1), bd);
+        }
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait_all();
     }
-    tc::wgmma_commit();
-    tc::wgmma_wait_all();
     tc::wgmma_fence_operand(d[0]);
     tc::wgmma_fence_operand(d[1]);
     tc::acc_store<N>(act, cD, tid, d);
@@ -78,18 +110,26 @@ __global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __rest
 extern "C" int nr_tc_selftest(const float* A, const float* W, float* D, int n, int k, int mode, void* stream) {
   NR_CHECK_ARG(A && W && D, "null pointer");
   cudaStream_t s = (cudaStream_t)stream;
-  auto run = [&](auto* fn1, auto* fn3, int k_) {
-    // the pass count is a template argument: a runtime loop around the wgmma batch makes ptxas serialise it
-    auto* fn = mode == 0 ? fn1 : fn3;
+  NR_CHECK_ARG(mode >= 0 && mode <= 2, "mode");
+  auto run = [&](auto* fn, int k_) {
     const int smem = (2 * k_ + 64) / 32 * 4096 * 4;
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     fn<<<1, 128, smem, s>>>(A, W, D);
   };
-  if (n == 32 && k == 32) run(nr::tc_selftest_kernel<32, 32, 1>, nr::tc_selftest_kernel<32, 32, 3>, 32);
-  else if (n == 64 && k == 64) run(nr::tc_selftest_kernel<64, 64, 1>, nr::tc_selftest_kernel<64, 64, 3>, 64);
-  else if (n == 16 && k == 64) run(nr::tc_selftest_kernel<16, 64, 1>, nr::tc_selftest_kernel<16, 64, 3>, 64);
-  else {
-    nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d", n, k);
+  // the mode is a template argument: a runtime loop around the wgmma batch makes ptxas serialise it
+  if (n == 32 && k == 32) {
+    if (mode == 0) run(nr::tc_selftest_kernel<32, 32, 0>, 32);
+    else if (mode == 1) run(nr::tc_selftest_kernel<32, 32, 1>, 32);
+    else run(nr::tc_selftest_kernel<32, 32, 2>, 32);
+  } else if (n == 64 && k == 64 && mode < 2) {
+    if (mode == 0) run(nr::tc_selftest_kernel<64, 64, 0>, 64);
+    else run(nr::tc_selftest_kernel<64, 64, 1>, 64);
+  } else if (n == 16 && k == 64) {
+    if (mode == 0) run(nr::tc_selftest_kernel<16, 64, 0>, 64);
+    else if (mode == 1) run(nr::tc_selftest_kernel<16, 64, 1>, 64);
+    else run(nr::tc_selftest_kernel<16, 64, 2>, 64);
+  } else {
+    nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d mode=%d", n, k, mode);
     return NR_E_UNSUPPORTED;
   }
   NR_CHECK_LAUNCH("tc_selftest");

@@ -44,18 +44,10 @@ p.use_vis, p.var_bias, p.point_rec = 0, 0.05, rec.data_ptr()
 _lib.check(_lib.lib().nr_point_kernel_timing(C.byref(p), timing.data_ptr(), None), "timing")
 torch.cuda.synchronize()
 t = timing.cpu().reshape(64, 2, 32)
-nm = ["geom+proj", "gather", "RF->A", "dd heads", "hit/vis+pe0", "pe1+nf+raydir", "pool1+base0 per point", "base0 epilogue", "base1",
-      "vis0", "vis1", "v20", "rgb0", "pool2+geo0 per point", "geo2 (wg0) / blend (wg1) + rec"]
+nm = ["geom+proj", "gather", "RF->A", "dd heads", "hit/vis+pe0", "pe1+nf+raydir", "pool1+base0 per point", "base0 epilogue",
+      "base1 (chain entry)", "vis0", "vis2+vis1", "v20+v21", "rgb0+exit", "pool2+geo0 per point", "geo2 (wg0) / blend (wg1) + rec"]
 for wg in (0, 1):
     d = (t[4:40, wg, 1:16] - t[4:40, wg, 0:15]).double().mean(0)
     tot = (t[4:40, wg, 15] - t[4:40, wg, 0]).double().mean()
     print(f"warp group {wg}: tile (16 points x 8 views = 128 rows) total {tot:.0f} cycles")
     print("  " + "  ".join(f"{nm[i]}:{d[i]:.0f}" for i in range(15)))
-# one layer's round trip (vis_fc.0): stamps 16.. = entry, A columns fenced, barrier, weights there, accumulators set up +
-# MMAs issued + committed, wgmma wait, accumulators stored + barrier + ring release, outputs loaded, epilogue computed,
-# next operand stored
-lbl = ["fence", "barrier", "wfull wait", "issue+commit", "mma wait", "acc store+barrier", "ld", "epilogue math", "st"]
-for wg in (0, 1):
-    m = t[4:40, wg, 16:26].double()
-    d = (m[:, 1:] - m[:, :-1]).mean(0)
-    print(f"warp group {wg} vis_fc.0 round trip: " + "  ".join(f"{lbl[i]}:{d[i]:.0f}" for i in range(9)) + f"  total {float((m[:, 9] - m[:, 0]).mean()):.0f}")
