@@ -117,31 +117,43 @@ static_assert(GRP_B % 4 == 0 && HOIST_W % 4 == 0 && BASE0_W % 4 == 0 && BASE1_W 
 
 // ------------------------------------------------------------------------------------------------------------
 // Tensor-core weight buffer (w_tc): every tensor-core layer's W^T as hi / lo tf32 parts, K padded and re-ordered to the
-// kernel's A-column order, pre-swizzled into K-major SWIZZLE_128B tiles of 32-wide K slabs, grouped into the 16 KB
-// ring stages the producer warp streams (offsets in floats).  Inside a stage:
-//   head h   : L0 hi 0 | L0 lo 1024 | L1 hi 2048 | L1 lo 3072                     (N 32, K 32)
-//   PE0      : hi slabs 0,1024 | lo slabs 2048,3072                              (N 32, K 34 -> 40)
-//   PE1      : hi 0 | lo 1024                                                     (N 32, K 32)
-//   B0 + s   : slab s of base_fc.0: hi 0 | lo 2048                                (N 64, K 67 -> 72 = 35+5 | 32)
-//   B1       : hi slabs 0,1024 | lo slabs 2048,3072                              (N 32, K 64)
-//   V01      : vis_fc.0 hi 0 | lo 1024 | vis_fc.2[:32] hi 2048 | lo 3072
-//   V2R      : vis_fc2.0 hi 0 | lo 1024 | rgb_fc.0 hi slabs 2048,2560 | lo slabs 3072,3584   (N 16, K 37 -> 40)
+// kernel's A-column order, pre-swizzled into K-major SWIZZLE_128B tiles of 32-wide K slabs (N rows x 32 floats), grouped
+// into the 16 KB ring stages the producer warp streams (offsets in floats).  Where a layer's parts sit inside its stage
+// or tile is a Tile below; the packer, the stage table and the kernel all read it from there.
 namespace tcl {
+// hi part at `hi`, lo part at `lo`, K slab s of either part s * slab floats further
+struct Tile {
+  int hi, lo, slab;
+};
 constexpr int STAGE = 4096;
-constexpr int HEAD0 = 0;
+constexpr int HEAD0 = 0;            // head h: stage h
+constexpr Tile HEAD_L0 = {0, 1024, 1024}, HEAD_L1 = {2048, 3072, 1024};   // N 32, K 32 each
 constexpr int PE0 = 4 * STAGE;
+constexpr Tile PE0_L = {0, 2048, 1024};                                    // N 32, K 34 -> 40
 constexpr int PE1 = PE0 + STAGE;
-constexpr int B0 = PE1 + STAGE;   // PE1 holds a 48-row tile (prob_embed.2 + neuray_fc.0 behind it): 3072 floats
+constexpr Tile PE1_L = {0, 1536, 1536};                                    // N 48 (prob_embed.2 + neuray_fc.0 behind it), K 32
+constexpr int PE1_SIZE = 3072;
+constexpr int B0 = PE1 + STAGE;     // base_fc.0's per-view inputs (rgb_feat 35 + bias + 4 zeros | neuray_feat 32): stage s holds slab s
+constexpr Tile B0_L = {0, 2048, STAGE};                                    // N 64, K 67 -> 72
 constexpr int B1 = B0 + 3 * STAGE;
+constexpr Tile B1_L = {0, 2048, 1024};                                     // N 32, K 64
 constexpr int V01 = B1 + STAGE;
+constexpr Tile VIS0_L = {0, 1024, 1024}, VIS2_L = {2048, 3072, 1024};      // vis_fc.0, vis_fc.2[:32]: N 32, K 32
 constexpr int V2R = V01 + STAGE;
-constexpr int RD1 = V2R + STAGE;    // ray_dir_fc.2 as a 48-row x K16 tile (hi 1536 | lo 1536), resident in shared memory
+constexpr Tile V20_L = {0, 1024, 1024}, RGB0_L = {2048, 3072, 512};        // vis_fc2.0: N 32, K 32; rgb_fc.0: N 16, K 37 -> 40
+constexpr int RD1 = V2R + STAGE;    // ray_dir_fc.2, resident in shared memory
+constexpr Tile RD1_L = {0, 1536, 1536};                                    // N 48 (35 used), K 16
 constexpr int RD1_SIZE = 3072;
-constexpr int HST = RD1 + RD1_SIZE;    // the 140 view-pooled inputs of base_fc.0 as a 64-row x K160 tile: hi 5 slabs | lo 5 slabs; K index
-constexpr int HST_SIZE = 2 * 5 * 2048; //   = 32*round + 8*stat + i  (feature 8*round + i; stat = mean0, var0, mean1, var1), resident in shared memory
-constexpr int G0 = HST + HST_SIZE;      // geometry_fc.0 on the view-pooled statistics: three ring stages (hi 2048 | lo 2048), 64 rows x K32 each;
-                                        //   K index = 32*round + 16*stat + i (feature 16*round + i; stat = mean, var); K 64 = mean weight, K 65 = bias
+constexpr int HST = RD1 + RD1_SIZE; // the 140 view-pooled inputs of base_fc.0: K index = 32*round + 8*stat + i (feature 8*round + i;
+                                    //   stat = mean0, var0, mean1, var1)
+constexpr Tile HST_L = {0, 10240, 2048};                                   // N 64, K 140 -> 160: hi 5 slabs | lo 5 slabs
+constexpr int HST_SIZE = 2 * HST_L.lo;
+constexpr Tile HST_STAGE = {0, 2048, 2048};   // HST streams through the ring a slab per stage: hi slab | lo slab right behind it
+constexpr int G0 = HST + HST_SIZE;  // geometry_fc.0 on the view-pooled statistics, stage s holds slab s: K index = 32*round +
+                                    //   16*stat + i (feature 16*round + i; stat = mean, var); K 64 = mean weight, K 65 = bias
+constexpr Tile G0_L = {0, 2048, STAGE};                                    // N 64, K 66 -> 96
 constexpr int TOTAL = G0 + 3 * STAGE;
+static_assert(HST_STAGE.lo == HST_L.slab, "stage_source lands a HST lo slab right behind its hi slab");
 }  // namespace tcl
 
 // ------------------------------------------------------------------------------------------------------------

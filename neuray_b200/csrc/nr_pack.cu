@@ -32,13 +32,12 @@ struct Out {
   float* wt;
 };
 
-// element (row n, column k) of a tensor-core tile: slab k/32 (slab_stride floats apart), swizzled inside; hi part at
-// `off`, lo part `lo_off` floats further
-__device__ __forceinline__ void put_tc(float* wt, int off, int lo_off, int slab_stride, int n, int k, float v) {
-  const int pos = off + (k >> 5) * slab_stride + tc::sw128_index(n, k & 31);
+// element (row n, column k) of the tensor-core tile at `off` with layout t: slab k/32, swizzled inside
+__device__ __forceinline__ void put_tc(float* wt, int off, tcl::Tile t, int n, int k, float v) {
+  const int pos = off + (k >> 5) * t.slab + tc::sw128_index(n, k & 31);
   const float hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-  wt[pos] = hi;
-  wt[pos + lo_off] = v - hi;
+  wt[pos + t.hi] = hi;
+  wt[pos + t.lo] = v - hi;
 }
 
 __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
@@ -57,7 +56,7 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
       const int r = e >> 5, k = e & 31;
       double acc = 0.0;
       for (int j = 0; j < 32; ++j) acc = fma(double(nf0[r * 32 + j]), double(pe1[j * 32 + k]), acc);
-      put_tc(wt, tcl::PE1, 1536, 48 * 32, 32 + r, k, float(acc));
+      put_tc(wt, tcl::PE1, tcl::PE1_L, 32 + r, k, float(acc));
     }
     return;
   }
@@ -68,39 +67,39 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
     if (job < 12) {
       const int h = job / 3, l = job - 3 * h;
       const int base = lay::DD_HEAD + h * lay::DD_HEAD_STRIDE;
-      if (l == 0) { wp[base + lay::DD_L0_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE, 1024, 1024, o, i, v); }
-      else if (l == 1) { wp[base + lay::DD_L1_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE + 2048, 1024, 1024, o, i, v); }
+      if (l == 0) { wp[base + lay::DD_L0_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L0, o, i, v); }
+      else if (l == 1) { wp[base + lay::DD_L1_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L1, o, i, v); }
       else wp[base + lay::DD_L2_W + o * 32 + i] = v;
       continue;
     }
     switch (job) {
-      case J_PE0: wp[lay::GRP_B + lay::PE0_W + i * 32 + o] = v; put_tc(wt, tcl::PE0, 2048, 1024, o, i, v); break;
-      case J_PE1: wp[lay::GRP_B + lay::PE1_W + i * 32 + o] = v; put_tc(wt, tcl::PE1, 1536, 48 * 32, o, i, v); break;
+      case J_PE0: wp[lay::GRP_B + lay::PE0_W + i * 32 + o] = v; put_tc(wt, tcl::PE0, tcl::PE0_L, o, i, v); break;
+      case J_PE1: wp[lay::GRP_B + lay::PE1_W + i * 32 + o] = v; put_tc(wt, tcl::PE1, tcl::PE1_L, o, i, v); break;
       case J_RD0: wp[lay::GRP_B + lay::RD0_W + i * 16 + o] = v; break;
-      case J_RD1: wp[lay::GRP_B + lay::RD1_W + i * 36 + o] = v; put_tc(wt, tcl::RD1, 1536, 48 * 32, o, i, v); break;
+      case J_RD1: wp[lay::GRP_B + lay::RD1_W + i * 36 + o] = v; put_tc(wt, tcl::RD1, tcl::RD1_L, o, i, v); break;
       case J_NF0: wp[lay::GRP_B + lay::NF0_W + i * 8 + o] = v; break;
       case J_NF1: wp[lay::GRP_B + lay::NF1_W + i] = v; break;
       case J_B0: {   // base_fc.0 [64,207] = [view-pooled 140 | rgb_feat 35 | neuray_feat 32]
         if (i < 140) {
           wp[lay::HOIST_W + i * 64 + o] = v;
           const int s = i / 35, f = i - 35 * s, r = f >> 3, q = f & 7;        // stat, feature -> K = 32 r + 8 s + q
-          put_tc(wt, tcl::HST, 10240, 2048, o, 32 * r + 8 * s + q, v);
+          put_tc(wt, tcl::HST, tcl::HST_L, o, 32 * r + 8 * s + q, v);
         } else {
           wp[lay::BASE0_W + (i - 140) * 64 + o] = v;
           const int k = i < 175 ? i - 140 : 40 + (i - 175);                    // rgb_feat 35 | bias | 4 zeros | neuray_feat 32
-          put_tc(wt, tcl::B0, 2048, tcl::STAGE, o, k, v);
+          put_tc(wt, tcl::B0, tcl::B0_L, o, k, v);
         }
         break;
       }
-      case J_B1: wp[lay::BASE1_W + i * 32 + o] = v; put_tc(wt, tcl::B1, 2048, 1024, o, i, v); break;
-      case J_V0: wp[lay::GRP_D1 + lay::VIS0_W + i * 32 + o] = v; put_tc(wt, tcl::V01, 1024, 1024, o, i, v); break;
+      case J_B1: wp[lay::BASE1_W + i * 32 + o] = v; put_tc(wt, tcl::B1, tcl::B1_L, o, i, v); break;
+      case J_V0: wp[lay::GRP_D1 + lay::VIS0_W + i * 32 + o] = v; put_tc(wt, tcl::V01, tcl::VIS0_L, o, i, v); break;
       case J_V1:
-        if (o < 32) { wp[lay::GRP_D1 + lay::VIS1_W + i * 32 + o] = v; put_tc(wt, tcl::V01 + 2048, 1024, 1024, o, i, v); }
+        if (o < 32) { wp[lay::GRP_D1 + lay::VIS1_W + i * 32 + o] = v; put_tc(wt, tcl::V01, tcl::VIS2_L, o, i, v); }
         else wp[lay::GRP_D1 + lay::VIS1L_W + i] = v;
         break;
-      case J_V20: wp[lay::GRP_D1 + lay::V20_W + i * 32 + o] = v; put_tc(wt, tcl::V2R, 1024, 1024, o, i, v); break;
+      case J_V20: wp[lay::GRP_D1 + lay::V20_W + i * 32 + o] = v; put_tc(wt, tcl::V2R, tcl::V20_L, o, i, v); break;
       case J_V21: wp[lay::GRP_D1 + lay::V21_W + i] = v; break;
-      case J_C0: wp[lay::GRP_D1 + lay::RGB0_W + i * 16 + o] = v; put_tc(wt, tcl::V2R + 2048, 1024, 512, o, i, v); break;
+      case J_C0: wp[lay::GRP_D1 + lay::RGB0_W + i * 16 + o] = v; put_tc(wt, tcl::V2R, tcl::RGB0_L, o, i, v); break;
       case J_C1: wp[lay::GRP_D1 + lay::RGB1_W + i * 8 + o] = v; break;
       case J_C2: wp[lay::GRP_D1 + lay::RGB2_W + i] = v; break;
       case J_G0: {   // geometry_fc.0 [64,65] = [mean 32 | var 32 | mean weight]
@@ -108,7 +107,7 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
         int k;
         if (i < 64) { const int s = i >> 5, f = i & 31, r = f >> 4, q = f & 15; k = 32 * r + 16 * s + q; }
         else k = 64;
-        put_tc(wt, tcl::G0, 2048, tcl::STAGE, o, k, v);
+        put_tc(wt, tcl::G0, tcl::G0_L, o, k, v);
         break;
       }
       case J_G1: wp[lay::GRP_D2 + lay::GEO1_W + i * 16 + o] = v; break;
@@ -140,7 +139,7 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
       case J_RD1: wp[lay::GRP_B + lay::RD1_B + o] = v; break;
       case J_NF0: wp[lay::GRP_B + lay::NF0_B + o] = v; break;
       case J_NF1: wp[lay::GRP_B + lay::NF1_B + o] = v; break;
-      case J_B0: wp[lay::HOIST_B + o] = v; put_tc(wt, tcl::B0, 2048, tcl::STAGE, o, 35, v); break;   // bias = column 35 (constant-1 input)
+      case J_B0: wp[lay::HOIST_B + o] = v; put_tc(wt, tcl::B0, tcl::B0_L, o, 35, v); break;   // bias = column 35 (constant-1 input)
       case J_B1: wp[lay::BASE1_B + o] = v; break;
       case J_V0: wp[lay::GRP_D1 + lay::VIS0_B + o] = v; break;
       case J_V1: wp[lay::GRP_D1 + (o < 32 ? lay::VIS1_B + o : lay::VIS1L_B)] = v; break;
@@ -149,7 +148,7 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
       case J_C0: wp[lay::GRP_D1 + lay::RGB0_B + o] = v; break;
       case J_C1: wp[lay::GRP_D1 + lay::RGB1_B + o] = v; break;
       case J_C2: wp[lay::GRP_D1 + lay::RGB2_B + o] = v; break;
-      case J_G0: wp[lay::GRP_D2 + lay::GEO0_B + o] = v; put_tc(wt, tcl::G0, 2048, tcl::STAGE, o, 65, v); break;   // bias = column 65
+      case J_G0: wp[lay::GRP_D2 + lay::GEO0_B + o] = v; put_tc(wt, tcl::G0, tcl::G0_L, o, 65, v); break;   // bias = column 65
       case J_G1: wp[lay::GRP_D2 + lay::GEO1_B + o] = v; break;
       case J_OG0: wr[lay::OG0_B + o] = v; break;
       case J_OG1: wr[lay::OG1_B + o] = v; break;

@@ -9,9 +9,10 @@
 //     tile by the row owners, W^T (hi / lo, pre-split and pre-swizzled by nr_pack_weights) sits in shared memory, the warp
 //     group multiplies them with wgmma and writes D back into the tile for the bias / activation epilogue, whose result
 //     goes back into the tile as the next A; warp group c issues the MMAs of rows 64c .. 64c + 63
-//   * weights stream through a 4 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk); full/empty
-//     mbarriers, the "empty" barrier takes one arrival from thread 0 of each compute warp group once that warp group's
-//     consuming wgmma have completed
+//   * weights stream through a 4 x 16 KB shared-memory ring filled by TMA bulk copies (cp.async.bulk) in the order of
+//     stage_source; full/empty mbarriers, the "empty" barrier takes one arrival from thread 0 of each compute warp group
+//     once that warp group's consuming wgmma have completed (Ring: the compute threads' side)
+//   * where each layer's B sits inside its ring stage is a tcl::Tile (nr_common.cuh), shared with the weight packer
 #include <type_traits>
 
 #include "nr_common.cuh"
@@ -51,15 +52,52 @@ __device__ __forceinline__ void load_stage(float* slot, const float* w_tc, int4 
 }
 
 // copies of stage s of a tile: heads, prob_embed x2, base_fc.0 x3, the view-pooled base_fc.0 inputs x5 (hi slab | lo slab
-// of the resident-layout HST tile), base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
+// of HST: tcl::HST_STAGE), base_fc.2, vis, vis2+rgb, geometry_fc.0 x3
 __device__ __forceinline__ int4 stage_source(int s, int n_heads) {
   if (s < n_heads) return make_int4(tcl::HEAD0 + s * RING_STAGE, RING_STAGE * 4, 0, 0);
   const int t = s - n_heads;
-  if (t >= 5 && t < 10) return make_int4(tcl::HST + (t - 5) * 2048, 2048 * 4, tcl::HST + tcl::HST_SIZE / 2 + (t - 5) * 2048, 2048 * 4);
+  if (t >= 5 && t < 10) {
+    const int slab = (t - 5) * tcl::HST_L.slab;
+    return make_int4(tcl::HST + tcl::HST_L.hi + slab, tcl::HST_L.slab * 4, tcl::HST + tcl::HST_L.lo + slab, tcl::HST_L.slab * 4);
+  }
   const int src = t == 0 ? tcl::PE0 : t == 1 ? tcl::PE1 : t <= 4 ? tcl::B0 + (t - 2) * RING_STAGE : t == 10 ? tcl::B1 : t == 11 ? tcl::V01
                 : t == 12 ? tcl::V2R : tcl::G0 + (t - 13) * RING_STAGE;
-  return make_int4(src, t == 1 ? 3072 * 4 : RING_STAGE * 4, 0, 0);
+  return make_int4(src, t == 1 ? tcl::PE1_SIZE * 4 : RING_STAGE * 4, 0, 0);
 }
+
+// The compute threads' side of the weight ring.  Stage i of the stream sits in slot i % NBUF, and a slot's barriers
+// complete once per trip round the ring, so stage i waits on parity (i / NBUF) & 1.  wi advances by the same amount in
+// every compute thread; only the leader arrives on `empty`, which counts one arrival per compute warp group.
+struct Ring {
+  struct Slot {
+    float* p;
+    uint32_t addr;              // shared-space byte address
+  };
+  float* base;                  // slot 0
+  uint32_t base_addr;
+  uint64_t *full, *empty;       // [NBUF] each
+  uint32_t wi;                  // stages consumed so far
+  bool leader;                  // thread 0 of the warp group: releases the stages for it
+  __device__ static uint32_t slot_of(uint32_t i) { return i % NBUF; }
+  __device__ static uint32_t parity(uint32_t i) { return (i / NBUF) & 1; }
+  // slot of stage wi + s
+  __device__ uint32_t slot_at(int s) const { return (slot_of(wi) + s) % NBUF; }
+  // where stage wi + s sits (without waiting for it)
+  __device__ Slot slot(int s) const {
+    const uint32_t k = slot_at(s);
+    return Slot{base + k * RING_STAGE, base_addr + k * (RING_STAGE * 4)};
+  }
+  // stage wi + s, once it has landed
+  __device__ Slot wait(int s) const {
+    tc::mbar_wait(full + slot_at(s), parity(wi + s));
+    return slot(s);
+  }
+  // this warp group is done with stage wi + s: its slot may be refilled
+  __device__ void release(int s) const {
+    if (leader) tc::mbar_arrive(empty + slot_at(s));
+  }
+  __device__ void advance(int n) { wi += n; }
+};
 
 // Everything a compute thread needs to drive its block's tensor-core layers.
 struct Blk {
@@ -68,10 +106,6 @@ struct Blk {
   int row;                      // this thread's row of the tile = its index in its warp group
   int wg;                       // compute warp group (0, 1): issues the MMAs of rows 64 wg .. 64 wg + 63, owns columns 4 wg + [0,4) of every 8
   int rbase, key;               // act_index(row, c + 4 wg) = (c >> 5) * 4096 + rbase + ((((c & 31) >> 2) ^ key) << 2) for c % 8 == 0
-  uint64_t *wfull, *wempty;     // arrays [NBUF]
-  uint32_t ring_addr;           // shared-space byte address of the ring
-  uint32_t wi;                  // weight stages consumed so far (same sequence in every thread)
-  bool leader;                  // thread 0 of the warp group: releases the ring stages for it
 };
 
 namespace pm {

@@ -10,8 +10,9 @@
 //     view-pooled statistics keep this split, because both pooled operands put one feature's statistics 8 or 16 columns
 //     apart.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0 only, each from the
 //     whole row in the tile.
-//   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer; both warp groups meet at a
-//     256-thread barrier before a layer (its A columns come from both) and after the accumulator store.  The dist-decoder
+//   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer, each layer as one 3xTF32 batch
+//     (mma_batch); both warp groups meet at a 256-thread barrier before a layer (its A columns come from both) and after
+//     the accumulator store (row_layer).  The dist-decoder
 //     heads (run_head) and the per-view tail base_fc.2 .. rgb_fc.0 (run_chain) are the exception: nothing in them is
 //     pooled or needs the row-owner layout, so each warp group runs them for its own 64 rows in the accumulator fragment
 //     (A from registers after the first layer, row sums over the 4 lanes that hold a row) and hands the results to the
@@ -102,17 +103,18 @@ struct PtAcc {
   static constexpr int MT = (PB + 15) / 16;
   float d[MT][3][4];
 };
-// acc += op[points][kcol + k] * W[8w + n][k], k < 8 KS: B from a weight ring stage `w` (64 rows x K32, K-major 128-byte
-// swizzle, hi slab | lo slab 2048 floats further, K steps 0 .. KS - 1).  Operand rows at or past PB read as 0.
+// acc += op[points][kcol + k] * W[8w + n][k], k < 8 KS: B from a weight ring stage `w` that holds one K32 slab of a 64-row
+// tile with layout L (K steps 0 .. KS - 1).  Operand rows at or past PB read as 0.
 template <int PB, int KS>
-__device__ __forceinline__ void point_mma(PtAcc<PB>& acc, const float* __restrict__ op, int kcol, const float* __restrict__ w, int warp, int lane) {
+__device__ __forceinline__ void point_mma(PtAcc<PB>& acc, const float* __restrict__ op, int kcol, const float* __restrict__ w, tcl::Tile L, int warp,
+                                          int lane) {
   const int g = lane >> 2, t = lane & 3;
-  const float* __restrict__ bw = w + warp * 256 + g * 32 + t;             // tc::sw128_index(8 warp + g, 8 j + t) = bw[((2j) ^ g) << 2]
+  const float* __restrict__ bw = w + L.hi + warp * 256 + g * 32 + t;      // tc::sw128_index(8 warp + g, 8 j + t) = bw[((2j) ^ g) << 2]
   const float* __restrict__ aw = op + g * OP_ROW + kcol + t;
 #pragma unroll
   for (int j = 0; j < KS; ++j) {
     const uint32_t bh[2] = {__float_as_uint(bw[((2 * j) ^ g) << 2]), __float_as_uint(bw[((2 * j + 1) ^ g) << 2])};
-    const uint32_t bl[2] = {__float_as_uint(bw[2048 + (((2 * j) ^ g) << 2)]), __float_as_uint(bw[2048 + (((2 * j + 1) ^ g) << 2)])};
+    const uint32_t bl[2] = {__float_as_uint(bw[L.lo - L.hi + (((2 * j) ^ g) << 2)]), __float_as_uint(bw[L.lo - L.hi + (((2 * j + 1) ^ g) << 2)])};
 #pragma unroll
     for (int m = 0; m < PtAcc<PB>::MT; ++m) {
       const bool ok0 = 16 * m + 8 <= PB || 16 * m + g < PB, ok1 = 16 * m + 16 <= PB || 16 * m + 8 + g < PB;
@@ -142,152 +144,95 @@ __device__ __forceinline__ void point_store(const PtAcc<PB>& acc, float* __restr
   }
 }
 
-// Layer issue, executed by both compute warp groups after they wrote their A columns; warp group c multiplies rows
-// 64c .. 64c + 63.  K chunk c (of NCH) reads A columns AHI + 8c (c < NLIN) or TAILHI + 8(c - NLIN), lo parts LOOFF
-// columns further, and B chunk CB0 + c of the layer's tiles (slab (CB0+c)/4; one ring stage per slab when NSTG > 1); ACC:
-// the first MMA accumulates onto what is already in the accumulator columns [DCOL, DCOL + N).  Returns with the outputs in
-// the activation tile, visible to every row owner of both warp groups.
-template <int N, int NCH, int AHI, int LOOFF, int NLIN, int TAILHI, int DCOL, int CB0, int NSTG, uint32_t OFF_HI, uint32_t OFF_LO,
-          uint32_t SLAB, bool WAIT_FULL, bool RELEASE, bool ACC>
-__device__ __forceinline__ void issue_layer(Blk& b) {
+// ---- tensor-core layers: one 3xTF32 wgmma batch each ----
+// A operand of a batch from the activation tile: K step c at column col + 8c, its lo part lo_off columns further, rows
+// 64 wg .. 64 wg + 63
+struct TileA {
+  uint32_t act_addr;
+  int wg, col, lo_off;
+  template <int KS>
+  __device__ void pin() const {}
+  __device__ uint64_t operator()(int c, bool lo) const { return tc::act_desc(act_addr, col + 8 * c + (lo ? lo_off : 0), wg); }
+};
+__device__ __forceinline__ TileA tile_a(const Blk& b, int col, int lo_off) { return TileA{b.act_addr, b.wg, col, lo_off}; }
+// A from registers (tc::wgmma_tf32_ra): K step c from h[c] / l[c].  The K steps a batch reads stay pinned until it has
+// completed.
+template <int KA>
+struct RegA {
+  uint32_t (&h)[KA][4];
+  uint32_t (&l)[KA][4];
+  template <int KS>
+  __device__ void pin() const {
+    tc::wgmma_fence_operand<KS>(h);
+    tc::wgmma_fence_operand<KS>(l);
+  }
+  __device__ const uint32_t (&operator()(int c, bool lo) const)[4] { return lo ? l[c] : h[c]; }
+};
+template <int N>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b) { tc::wgmma_tf32<N>(d, a, b); }
+template <int N>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b) { tc::wgmma_tf32_ra<N>(d, a, b); }
+// B operand of a batch in a tensor-core tile (tcl::Tile t) at shared byte address `addr`: K step c is step c & 3 of slab c >> 2
+struct TileB {
+  uint64_t hi, lo;
+  int slab16;                   // slab stride in 16-byte descriptor units
+  __device__ uint64_t operator()(int c, bool l) const { return (l ? lo : hi) + (c >> 2) * slab16 + 2 * (c & 3); }
+};
+__device__ __forceinline__ TileB tile_b(uint32_t addr, tcl::Tile t) {
+  return TileB{tc::smem_desc_sw128(addr + t.hi * 4), tc::smem_desc_sw128(addr + t.lo * 4), t.slab / 4};
+}
+// B of base_fc.0's per-view inputs from its K step k0 on: slab s of tcl::B0_L is ring stage wi + s
+__device__ __forceinline__ auto base0_b(const Ring& ring, int k0) {
+  return [=](int c, bool lo) {
+    const int k = k0 + c;
+    return tc::smem_desc_sw128(ring.slot(k >> 2).addr + (lo ? tcl::B0_L.lo : tcl::B0_L.hi) * 4) + 2 * (k & 3);
+  };
+}
+
+// d (+)= A x B over K steps c < KS, issued by this warp group as one wgmma batch and waited for; `under` runs between the
+// commit and the wait.  Every batch of the kernel goes through here, so every accumulator gets its products in the same
+// order: pass hi*hi, lo*hi, hi*lo, the K steps inside each pass.  a(c, lo) (TileA or RegA) and bd(c, lo): the A operand
+// and the B descriptor of K step c, hi or lo part.  ACC: onto what d holds, else from 0.
+template <int N, int KS, bool ACC = false, class A, class B, class U>
+__device__ __forceinline__ void mma_batch(float (&d)[N / 2], const A& a, const B& bd, U&& under) {
+  if (!ACC) {
+#pragma unroll
+    for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
+  }
+  tc::wgmma_fence_operand(d);
+  a.template pin<KS>();
+  tc::wgmma_fence();
+#pragma unroll
+  for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
+    for (int c = 0; c < KS; ++c) wgmma<N>(d, a(c, ps == 1), bd(c, ps == 2));
+  }
+  tc::wgmma_commit();
+  under();
+  tc::wgmma_wait_all();
+  tc::wgmma_fence_operand(d);
+  a.template pin<KS>();
+}
+
+// A row-owner layer, executed by both compute warp groups after they wrote their A columns; warp group c multiplies rows
+// 64c .. 64c + 63.  b_ready() runs once both are at the layer: it waits for the B operand's ring stages, if any, and
+// returns its descriptors.  ACC: onto what the accumulator columns [DCOL, DCOL + N) hold.  Returns with the outputs in
+// those columns, visible to every row owner of both warp groups, and both warp groups' reads of B completed.
+template <int N, int KS, int DCOL, bool ACC, class BReady>
+__device__ __forceinline__ void row_layer(const Blk& b, const TileA& a, BReady&& b_ready) {
   tc::fence_proxy_async_smem();              // this thread's A columns -> visible to the tensor cores
   tc::named_sync(BAR_LAYER, NCOMP);
-  const uint32_t st0 = b.wi % NBUF;
-  if (WAIT_FULL) {
-#pragma unroll
-    for (int s = 0; s < NSTG; ++s) tc::mbar_wait(b.wfull + ((st0 + s) % NBUF), ((b.wi + s) / NBUF) & 1);
-  }
+  const auto bd = b_ready();
   float d[N / 2];
   if (ACC) tc::acc_load_half<N>(b.act, DCOL, b.row, b.wg, d);
-  else {
-#pragma unroll
-    for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
-  }
-  uint64_t dhi[NSTG], dlo[NSTG];
-#pragma unroll
-  for (int s = 0; s < NSTG; ++s) {
-    const uint32_t base = b.ring_addr + ((st0 + s) % NBUF) * (RING_STAGE * 4);
-    dhi[s] = tc::smem_desc_sw128(base + OFF_HI);
-    dlo[s] = tc::smem_desc_sw128(base + OFF_LO);
-  }
-  tc::wgmma_fence_operand(d);
-  tc::wgmma_fence();
-#pragma unroll
-  for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int acol = (c < NLIN ? AHI + 8 * c : TAILHI + 8 * (c - NLIN)) + (ps == 1 ? LOOFF : 0);
-      const int cb = CB0 + c;
-      const int slab = cb >> 2;
-      const int stg = NSTG == 1 ? 0 : slab;
-      const uint32_t inc = ((NSTG == 1 ? slab * SLAB : 0u) + (cb & 3) * 32) >> 4;
-      const uint64_t bd = (ps == 2 ? dlo[stg] : dhi[stg]) + inc;
-      tc::wgmma_tf32<N>(d, tc::act_desc(b.act_addr, acol, b.wg), bd);
-    }
-  }
-  tc::wgmma_commit();
-  tc::wgmma_wait_all();
-  tc::wgmma_fence_operand(d);
-  tc::acc_store_half<N>(b.act, DCOL, b.row, b.wg, d);
-  tc::named_sync(BAR_LAYER, NCOMP);          // outputs in the tile; both warp groups' reads of the stages have completed
-  if (RELEASE) {
-    if (b.leader) {
-#pragma unroll
-      for (int s = 0; s < NSTG; ++s) tc::mbar_arrive(b.wempty + ((st0 + s) % NBUF));
-    }
-    b.wi += NSTG;
-  }
-}
-// Same, B operand = a resident shared-memory tile at byte address `base` (hi slabs first, SLAB bytes apart; lo parts
-// OFF_LO bytes further): no ring accounting.
-template <int N, int NCH, int AHI, int LOOFF, int DCOL, int CB0, uint32_t OFF_LO, uint32_t SLAB, bool ACC>
-__device__ __forceinline__ void issue_layer_resident(Blk& b, uint32_t base) {
-  tc::fence_proxy_async_smem();
-  tc::named_sync(BAR_LAYER, NCOMP);
-  float d[N / 2];
-  if (ACC) tc::acc_load_half<N>(b.act, DCOL, b.row, b.wg, d);
-  else {
-#pragma unroll
-    for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
-  }
-  const uint64_t dhi = tc::smem_desc_sw128(base), dlo = tc::smem_desc_sw128(base + OFF_LO);
-  tc::wgmma_fence_operand(d);
-  tc::wgmma_fence();
-#pragma unroll
-  for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int acol = AHI + 8 * c + (ps == 1 ? LOOFF : 0);
-      const int cb = CB0 + c;
-      const uint32_t inc = ((cb >> 2) * SLAB + (cb & 3) * 32) >> 4;
-      const uint64_t bd = (ps == 2 ? dlo : dhi) + inc;
-      tc::wgmma_tf32<N>(d, tc::act_desc(b.act_addr, acol, b.wg), bd);
-    }
-  }
-  tc::wgmma_commit();
-  tc::wgmma_wait_all();
-  tc::wgmma_fence_operand(d);
+  mma_batch<N, KS, ACC>(d, a, bd, [] {});
   tc::acc_store_half<N>(b.act, DCOL, b.row, b.wg, d);
   tc::named_sync(BAR_LAYER, NCOMP);
-}
-// the common case: activations hi [0,64) / lo [64,128), accumulator at 128, one ring stage
-template <int N, int NCH, int AHI, int NLIN, int TAILHI, uint32_t OFF_HI, uint32_t OFF_LO, uint32_t SLAB, bool WAIT_FULL, bool RELEASE>
-__device__ __forceinline__ void run_layer(Blk& b) {
-  issue_layer<N, NCH, AHI, 64, NLIN, TAILHI, 128, 0, 1, OFF_HI, OFF_LO, SLAB, WAIT_FULL, RELEASE, false>(b);
 }
 
 // ---- layers in the accumulator fragment of the warp group that issues them (the heads and the per-view chain) ----
 // This thread holds columns 8j + 2q + {0, 1} of fragment rows fr and fr + 8 (q = t % 4, tc::acc_load_half):
-// d[4j + 2r + e] is column 8j + 2q + e of row fr + 8r.  B of K step c sits at descriptor + (c >> 2) SLAB16 + 2 (c & 3)
-// of the hi (passes 0, 1) or lo (pass 2) descriptor; the passes and K steps go in issue_layer's order, so the
-// accumulators get the same products in the same order as a round trip through the tile.
-// d = A x B, A = tile columns [0, 8 KS) (hi) / [64, 64 + 8 KS) (lo) of this warp group's 64 rows.  Committed, not waited for.
-template <int KS, int SLAB16>
-__device__ __forceinline__ void issue_frag_ss(const Blk& b, float (&d)[16], uint64_t dhi, uint64_t dlo) {
-#pragma unroll
-  for (int j = 0; j < 16; ++j) d[j] = 0.f;
-  tc::wgmma_fence_operand(d);
-  tc::wgmma_fence();
-#pragma unroll
-  for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-    for (int c = 0; c < KS; ++c)
-      tc::wgmma_tf32<32>(d, tc::act_desc(b.act_addr, 8 * c + (ps == 1 ? 64 : 0), b.wg), (ps == 2 ? dlo : dhi) + (c >> 2) * SLAB16 + 2 * (c & 3));
-  }
-  tc::wgmma_commit();
-}
-// d = A x B, A from registers: K step c from ah[c] / al[c] (c < KS <= KA).  Committed, not waited for: the A registers and
-// d stay pinned until wait_frag.
-template <int N, int KS, int SLAB16, int KA>
-__device__ __forceinline__ void issue_frag_ra(float (&d)[N / 2], uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4], uint64_t dhi, uint64_t dlo) {
-#pragma unroll
-  for (int j = 0; j < N / 2; ++j) d[j] = 0.f;
-  tc::wgmma_fence_operand(d);
-#pragma unroll
-  for (int c = 0; c < KS; ++c)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ah[c][i]), "+r"(al[c][i])::"memory");
-  tc::wgmma_fence();
-#pragma unroll
-  for (int ps = 0; ps < 3; ++ps) {
-#pragma unroll
-    for (int c = 0; c < KS; ++c) tc::wgmma_tf32_ra<N>(d, ps == 1 ? al[c] : ah[c], (ps == 2 ? dlo : dhi) + (c >> 2) * SLAB16 + 2 * (c & 3));
-  }
-  tc::wgmma_commit();
-}
-template <int N, int KS, int KA>
-__device__ __forceinline__ void wait_frag_ra(float (&d)[N / 2], uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4]) {
-  tc::wgmma_wait_all();
-  tc::wgmma_fence_operand(d);
-#pragma unroll
-  for (int c = 0; c < KS; ++c)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(ah[c][i]), "+r"(al[c][i])::"memory");
-}
-__device__ __forceinline__ void wait_frag(float (&d)[16]) {
-  tc::wgmma_wait_all();
-  tc::wgmma_fence_operand(d);
-}
+// d[4j + 2r + e] is column 8j + 2q + e of row fr + 8r.
 // An N = 32 fragment x (after its epilogue) -> the A fragments of the next layer's 4 K steps, split into hi / lo
 // (ah[j], al[j], j < 4).  A K step wants columns 8j + q and 8j + q + 4 of rows fr, fr + 8 (tc::wgmma_tf32_ra): lane q of
 // a quad reads lane s = 2 (q & 1) + (q >> 1) in the first shuffle and lane s ^ 2 in the second; a lane offers column
@@ -329,17 +274,12 @@ __device__ __forceinline__ void row_dot(const float (&z)[16], const float* __res
 // One dist-decoder head (two K 32, N 32 layers and the (o0, o1) outputs) for the 64 rows whose MMAs this warp group
 // issues, without leaving its registers and without meeting the other warp group: L0 reads A[0:32] from the tile (both
 // warp groups wrote it before the barrier in front of the heads), its epilogue runs on the accumulator fragment, L1 takes
-// A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  Releases the head's ring stage on its own
-// (wempty counts one arrival per compute warp group).
-__device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, float* __restrict__ xo, int fr) {
+// A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  Releases the head's ring stage on its own.
+__device__ __forceinline__ void run_head(const Blk& b, Ring& ring, const float* __restrict__ hw, float* __restrict__ xo, int fr) {
   const int lane = b.row & 31, q = lane & 3;
-  const uint32_t st = b.wi % NBUF;
-  tc::mbar_wait(b.wfull + st, (b.wi / NBUF) & 1);
-  const uint32_t base = b.ring_addr + st * (RING_STAGE * 4);
-  // L0: B hi / lo at stage floats 0 / 1024
+  const uint32_t w = ring.wait(0).addr;
   float d[16];
-  issue_frag_ss<4, 0>(b, d, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
-  wait_frag(d);
+  mma_batch<32, 4>(d, tile_a(b, 0, 64), tile_b(w, tcl::HEAD_L0), [] {});
   // bias + ELU, then into L1's A layout
   uint32_t ah[4][4], al[4][4];
 #pragma unroll
@@ -352,12 +292,10 @@ __device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, f
     }
   }
   frag_to_a(d, lane, ah, al);
-  // L1: B hi / lo at stage floats 2048 / 3072
   float e[16];
-  issue_frag_ra<32, 4, 0>(e, ah, al, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
-  wait_frag_ra<32, 4>(e, ah, al);
-  if (b.leader) tc::mbar_arrive(b.wempty + st);
-  b.wi += 1;
+  mma_batch<32, 4>(e, RegA<4>{ah, al}, tile_b(w, tcl::HEAD_L1), [] {});
+  ring.release(0);
+  ring.advance(1);
   // (o0, o1) of rows fr, fr + 8: this thread's 8 columns, then the quad's sum; lane q stores output q & 1 of row fr + 8 (q >> 1)
   float p[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -388,34 +326,26 @@ __device__ __forceinline__ void run_head(Blk& b, const float* __restrict__ hw, f
 // A from registers.  vis_fc.1 and vis_fc2.1 are summed by the quad that holds a row, in column order (row_dot), so every
 // value is bit-identical to a round trip through the row owners.  Leaves x2 (base_fc.2's output +
 // the vis_fc residual) in tile columns [96,128), rgb_fc.0's pre-activations in [128,144) and vis2 in xch slot XCH_L2.
-// Ring stages (each warp group waits and releases on its own): base_fc.2 | vis_fc.0 (B hi / lo at stage floats
-// 0 / 1024) + vis_fc.2 (2048 / 3072) | vis_fc2.0 (0 / 1024) + rgb_fc.0 (2048 / 3072, K step 4 512 floats further).
+// Ring stages (each warp group waits and releases on its own): base_fc.2 (tcl::B1_L) | vis_fc.0 + vis_fc.2 (tcl::VIS0_L,
+// VIS2_L) | vis_fc2.0 + rgb_fc.0 (tcl::V20_L, RGB0_L).
 // tk: where the phase stamps after base_fc.2, vis_fc.0, vis_fc.2 and vis_fc2.0 go (nullptr: none).
-__device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, float* __restrict__ xch, int fr, long long* tk) {
+__device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float* __restrict__ sw, float* __restrict__ xch, int fr, long long* tk) {
   const int lane = b.row & 31, q = lane & 3;
-  auto stage = [&](int s) {
-    const uint32_t i = b.wi + s;
-    tc::mbar_wait(b.wfull + i % NBUF, (i / NBUF) & 1);
-    return b.ring_addr + (i % NBUF) * (RING_STAGE * 4);
-  };
-  auto release = [&](int s) {
-    if (b.leader) tc::mbar_arrive(b.wempty + (b.wi + s) % NBUF);
-  };
   // base_fc.2: K = 64 from the tile; the row scalars load under its MMAs
-  uint32_t base = stage(0);
+  uint32_t w = ring.wait(0).addr;
   float d[16];
-  issue_frag_ss<8, 256>(b, d, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 2048 * 4));
   float w1[2], mr[2], t0[2], t1[2];                 // t0, t1: rgb_fc.0's K tail, columns 32 + q and 36 + q (t0 of lane 0 is vis2)
+  mma_batch<32, 8>(d, tile_a(b, 0, 64), tile_b(w, tcl::B1_L), [&] {
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const float* __restrict__ x = xch + XCH_ROW * 128 + fr + 8 * r;
-    w1[r] = x[0];
-    mr[r] = x[128];
-    t0[r] = q == 0 ? 0.f : x[(1 + q) * 128];
-    t1[r] = q == 0 ? x[5 * 128] : 0.f;
-  }
-  wait_frag(d);
-  release(0);
+    for (int r = 0; r < 2; ++r) {
+      const float* __restrict__ x = xch + XCH_ROW * 128 + fr + 8 * r;
+      w1[r] = x[0];
+      mr[r] = x[128];
+      t0[r] = q == 0 ? 0.f : x[(1 + q) * 128];
+      t1[r] = q == 0 ? x[5 * 128] : 0.f;
+    }
+  });
+  ring.release(0);
   float xr[16];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -430,9 +360,8 @@ __device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, 
   frag_to_a(xr, lane, ah, al);
   if (tk) tk[0] = clock64();
   // vis_fc.0 (row scale w1 in the epilogue)
-  base = stage(1);
-  issue_frag_ra<32, 4, 0>(d, ah, al, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
-  wait_frag_ra<32, 4>(d, ah, al);
+  w = ring.wait(1).addr;
+  mma_batch<32, 4>(d, RegA<4>{ah, al}, tile_b(w, tcl::VIS0_L), [] {});
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const float2 bb = *reinterpret_cast<const float2*>(sw + SW_V0B + 8 * j + 2 * q);
@@ -446,9 +375,8 @@ __device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, 
   if (tk) tk[1] = clock64();
   // vis_fc.2, then vis_fc.1 (the vis_fc.0 outputs' dot product; under the MMAs, with their A registers pinned, it spills)
   float e[16];
-  issue_frag_ra<32, 4, 0>(e, ah, al, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
-  wait_frag_ra<32, 4>(e, ah, al);
-  release(1);
+  mma_batch<32, 4>(e, RegA<4>{ah, al}, tile_b(w, tcl::VIS2_L), [] {});
+  ring.release(1);
   float visa[2];
   {
     float lg[2];
@@ -470,10 +398,8 @@ __device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, 
   frag_to_a(xr, lane, a2h, a2l);
   if (tk) tk[2] = clock64();
   // vis_fc2.0; x2 goes to the tile under its MMAs
-  base = stage(2);
-  issue_frag_ra<32, 4, 0>(d, a2h, a2l, tc::smem_desc_sw128(base), tc::smem_desc_sw128(base + 1024 * 4));
-  tc::acc_store_half<32>(b.act, 96, b.row, b.wg, xr);
-  wait_frag_ra<32, 4>(d, a2h, a2l);
+  w = ring.wait(2).addr;
+  mma_batch<32, 4>(d, RegA<5>{a2h, a2l}, tile_b(w, tcl::V20_L), [&] { tc::acc_store_half<32>(b.act, 96, b.row, b.wg, xr); });
   float vis2[2];
   {
 #pragma unroll
@@ -498,11 +424,11 @@ __device__ __forceinline__ void run_chain(Blk& b, const float* __restrict__ sw, 
     tc::split_tf32(t1[r], a2h[4][2 + r], a2l[4][2 + r]);
   }
   float g[8];
-  issue_frag_ra<16, 5, 128>(g, a2h, a2l, tc::smem_desc_sw128(base + 2048 * 4), tc::smem_desc_sw128(base + 3072 * 4));
-  if (q < 2) xch[XCH_L2 * 128 + fr + 8 * q] = q ? vis2[1] : vis2[0];
-  wait_frag_ra<16, 5>(g, a2h, a2l);
-  release(2);
-  b.wi += 3;
+  mma_batch<16, 5>(g, RegA<5>{a2h, a2l}, tile_b(w, tcl::RGB0_L), [&] {
+    if (q < 2) xch[XCH_L2 * 128 + fr + 8 * q] = q ? vis2[1] : vis2[0];
+  });
+  ring.release(2);
+  ring.advance(3);
   tc::acc_store_half<16>(b.act, 128, b.row, b.wg, g);
 }
 
@@ -565,7 +491,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   const NrPassParams& pp = kp.p;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
-  float* const ring = smem + OFF_RING;
+  float* const ring_smem = smem + OFF_RING;
   float* const sWg1 = smem + OFF_WG1;
   float* const sw = smem + OFF_SW;
   uint64_t* const bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -630,9 +556,9 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       const uint32_t total = uint32_t(iters) * uint32_t(stages_per_tile);
       int s = 0;
       for (uint32_t n = 0; n < total; ++n) {
-        const uint32_t buf = n % NBUF;
-        if (n >= NBUF) tc::mbar_wait(wempty + buf, ((n / NBUF) - 1) & 1);
-        load_stage(ring + buf * RING_STAGE, pp.w_tc, table[s], wfull + buf);
+        const uint32_t buf = Ring::slot_of(n);
+        if (n >= NBUF) tc::mbar_wait(wempty + buf, Ring::parity(n - NBUF));   // both compute warp groups released stage n - NBUF
+        load_stage(ring_smem + buf * RING_STAGE, pp.w_tc, table[s], wfull + buf);
         if (++s == stages_per_tile) s = 0;
       }
     }
@@ -666,10 +592,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   b.wg = tid >> 7;
   b.rbase = (b.row >> 3) * 256 + (b.row & 7) * 32;
   b.key = (b.row & 7) ^ b.wg;
-  b.leader = b.row == 0;
-  b.wfull = wfull; b.wempty = wempty;
-  b.ring_addr = tc::smem_u32(ring);
-  b.wi = 0;
+  Ring ring{ring_smem, tc::smem_u32(ring_smem), wfull, wempty, 0, b.row == 0};
   const int row = b.row, wg = b.wg;
   const int fr = 64 * wg + 16 * (row >> 5) + ((row & 31) >> 2);           // this thread's accumulator fragment rows: fr, fr + 8
   // a point's 16 pooled values (which every lane of the point holds) -> its row of the per-point operand: value 4q + i at
@@ -694,13 +617,10 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     if (tile >= n_tiles) {
       // nothing to render in this iteration: still take part in the weight-ring accounting
       for (int s = 0; s < stages_per_tile; ++s) {
-        if (b.leader) {
-          const uint32_t i = b.wi + s;
-          tc::mbar_wait(wfull + (i % NBUF), (i / NBUF) & 1);
-          tc::mbar_arrive(wempty + (i % NBUF));
-        }
+        if (ring.leader) ring.wait(s);
+        ring.release(s);
       }
-      b.wi += stages_per_tile;
+      ring.advance(stages_per_tile);
       continue;
     }
     const int n = tile * PB + pl;
@@ -853,7 +773,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     tc::fence_proxy_async_smem();
     tc::named_sync(BAR_LAYER, NCOMP);
 #pragma unroll 1
-    for (int hd = 0; hd < n_heads; ++hd) run_head(b, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
+    for (int hd = 0; hd < n_heads; ++hd) run_head(b, ring, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
     PM_TICK(4)
     tc::named_sync(BAR_LAYER, NCOMP);                                              // head outputs -> the row owners
     // hit and visibility go into warp group 0's columns
@@ -890,7 +810,10 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       if (wg == 0) { x[0] = (hit - 0.5f) * 2.f; x[1] = (visib - 0.5f) * 2.f; }
       st_own<1>(b, 32, 96, x);                                                     // A[32:40] = hit', vis', 0... (the heads' hidden layer is dead)
     }
-    run_layer<32, 5, 0, 4, 32, 0, 2048 * 4, 4096, true, true>(b);                 // prob_embed.0: K = 32 + 8
+    // prob_embed.0: K = 32 + 8, accumulator columns [128,160)
+    row_layer<32, 5, 128, false>(b, tile_a(b, 0, 64), [&] { return tile_b(ring.wait(0).addr, tcl::PE0_L); });
+    ring.release(0);
+    ring.advance(1);
     {
       float x[16];
       ld_own<4>(b, 128, x);
@@ -901,7 +824,9 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     }
     PM_TICK(5)
     // prob_embed.2 with neuray_fc.0 behind it: N = 48, accumulator columns [96,144)
-    issue_layer<48, 4, 0, 64, 4, 0, 96, 0, 1, 0, 1536 * 4, 0, true, true, false>(b);
+    row_layer<48, 4, 96, false>(b, tile_a(b, 0, 64), [&] { return tile_b(ring.wait(0).addr, tcl::PE1_L); });
+    ring.release(0);
+    ring.advance(1);
     float gate;
     {
       float x[16];
@@ -914,8 +839,14 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) gate = fmaf(sw[SW_NF1W + j], elu(h8[j] + sw[SW_NF0C + j]), gate);
     }
-    // base_fc.0, K round A: the neuray_feat inputs (B chunks 5..8), accumulator columns [96,160)
-    issue_layer<64, 4, 0, 64, 4, 0, 96, 5, 3, 0, 2048 * 4, 0, true, false, false>(b);
+    // base_fc.0, K round A: the neuray_feat inputs (its K steps 5..8), accumulator columns [96,160); waits for all three
+    // of its stages, which round B reads too
+    row_layer<64, 4, 96, false>(b, tile_a(b, 0, 64), [&] {
+      ring.wait(0);
+      ring.wait(1);
+      ring.wait(2);
+      return base0_b(ring, 5);
+    });
     // rgb_feat (35) + zero padding: rf[4q + i] = column 8q + 4wg + i
     float rf[20];
     {
@@ -932,7 +863,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         }
         st_own<2>(b, 48, 64, h8);                                                  // ray_dir_fc.2 operand: hi [48,64), lo [64,80)
       }
-      issue_layer_resident<48, 2, 48, 16, 0, 0, 1536 * 4, 0, false>(b, tc::smem_u32(smem + OFF_RD1));   // ray_dir_fc.2: K = 16, accumulator [0,48)
+      // ray_dir_fc.2: K = 16, accumulator [0,48)
+      row_layer<48, 2, 0, false>(b, tile_a(b, 48, 16), [&] { return tile_b(tc::smem_u32(smem + OFF_RD1), tcl::RD1_L); });
       ld_own<5>(b, 0, rf);
       // + [rgb | img_feats]: column c holds img_feats channel c - 3, which warp group ((c - 3) >> 2) & 1 gathered into
       // its buffer column 4 ((c - 3) >> 3) + ((c - 3) & 3).  Of this warp group's columns 8q + 4wg + i, i = 3 is in its own
@@ -962,8 +894,11 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       }
       st_own<5>(b, 0, 48, rf);                                                     // rgb_feat: hi [0,40), lo [48,88)
     }
-    // base_fc.0, K round B: rgb_feat (B chunks 0..4)
-    issue_layer<64, 5, 0, 48, 5, 0, 96, 0, 3, 0, 2048 * 4, 0, false, true, true>(b);
+    // base_fc.0, K round B: rgb_feat (its K steps 0..4), onto round A's accumulators
+    row_layer<64, 5, 96, true>(b, tile_a(b, 0, 48), [&] { return base0_b(ring, 0); });
+#pragma unroll
+    for (int s = 0; s < 3; ++s) ring.release(s);
+    ring.advance(3);
     if (DEBUG && kp.dbg != nullptr && row_ok && wg == 0) {
       float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
       o[0] = mrow; o[1] = zrow; o[2] = hit; o[3] = visib; o[4] = dbg_px; o[5] = dbg_py;
@@ -976,7 +911,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     // round (statistic t of feature i at column 32 R + 8t + i, so warp group c pools features 4c .. 4c + 3 of the round).
     // They go into the point's row of the per-point operand (PB rows, K 160) and each round's K 32 is multiplied as soon
     // as it is complete, B from the round's ring stage, into a per-point [PB][64] result that the epilogue adds to every
-    // view's row.  One barrier per round: it publishes the round's operand columns and tells the leaders (b.leader) that every
+    // view's row.  One barrier per round: it publishes the round's operand columns and tells the leaders (Ring::leader) that every
     // warp is done with the previous round's stage (the fifth stage can only load into the first one's ring slot).  The sums over
     // the views go through the warp's transposition buffer (pool_rows); the variance comes from the weighted second moment:
     //   sum_v w (x - mu)^2 = sum_v w x^2 - mu^2 (2 - sum_v w),  mu = sum_v w x   (the reference's mean is NOT normalised)
@@ -986,7 +921,6 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     {
       const float c1 = 2.f - gsum(w1), c0 = 2.f - gsum(w0);
       float* const op = b.act;
-      const uint32_t s0 = b.wi;
       PtAcc<PB> acc = {};
       auto round = [&](auto rc) {
         constexpr int R = decltype(rc)::value;
@@ -1005,16 +939,15 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         }
         put_point(op, 32 * R, st);
         tc::named_sync(BAR_LAYER, NCOMP);
-        if (R > 0 && b.leader) tc::mbar_arrive(wempty + (s0 + R - 1) % NBUF);
-        tc::mbar_wait(wfull + (s0 + R) % NBUF, ((s0 + R) / NBUF) & 1);
-        point_mma<PB, 4>(acc, op, 32 * R, ring + ((s0 + R) % NBUF) * RING_STAGE, warp, lane);
+        if (R > 0) ring.release(R - 1);
+        point_mma<PB, 4>(acc, op, 32 * R, ring.wait(R).p, tcl::HST_STAGE, warp, lane);
       };
       round(std::integral_constant<int, 0>{}); round(std::integral_constant<int, 1>{}); round(std::integral_constant<int, 2>{});
       round(std::integral_constant<int, 3>{}); round(std::integral_constant<int, 4>{});
       point_store(acc, smem + OFF_PT, warp, lane);
       tc::named_sync(BAR_LAYER, NCOMP);                                            // per-point result visible; the last stage read
-      if (b.leader) tc::mbar_arrive(wempty + (s0 + 4) % NBUF);
-      b.wi += 5;
+      ring.release(4);
+      ring.advance(5);
     }
 
     PM_TICK(7)
@@ -1045,7 +978,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       if constexpr (DEBUG) {
         if (kp.timing != nullptr && blockIdx.x == 0 && row == 0 && it < 64) tk = kp.timing + (it * 2 + wg) * 32 + 9;
       }
-      run_chain(b, sw, xch, fr, tk);
+      run_chain(b, ring, sw, xch, fr, tk);
     }
     tc::named_sync(BAR_LAYER, NCOMP);                                              // x2, rgb_fc.0 and vis2 -> the row owners
     float xr[16];
@@ -1084,22 +1017,18 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         *reinterpret_cast<float4*>(op + pl * OP_ROW + 68) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
       tc::named_sync(BAR_LAYER, NCOMP);
-      const uint32_t s0 = b.wi;
       PtAcc<PB> acc = {};
 #pragma unroll
       for (int s = 0; s < 3; ++s) {
-        tc::mbar_wait(wfull + (s0 + s) % NBUF, ((s0 + s) / NBUF) & 1);
-        const float* w = ring + ((s0 + s) % NBUF) * RING_STAGE;
-        if (s < 2) point_mma<PB, 4>(acc, op, 32 * s, w, warp, lane);
-        else point_mma<PB, 1>(acc, op, 64, w, warp, lane);
+        const float* w = ring.wait(s).p;
+        if (s < 2) point_mma<PB, 4>(acc, op, 32 * s, w, tcl::G0_L, warp, lane);
+        else point_mma<PB, 1>(acc, op, 64, w, tcl::G0_L, warp, lane);
       }
       point_store(acc, smem + OFF_PT, warp, lane);
       tc::named_sync(BAR_LAYER, NCOMP);                                            // per-point result visible; the stages read
-      if (b.leader) {
 #pragma unroll
-        for (int s = 0; s < 3; ++s) tc::mbar_arrive(wempty + (s0 + s) % NBUF);
-      }
-      b.wi += 3;
+      for (int s = 0; s < 3; ++s) ring.release(s);
+      ring.advance(3);
     }
 
     PM_TICK(14)

@@ -61,9 +61,6 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 }
 // named barrier among `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
-// arrive on a named barrier without waiting: the shared-memory writes before it are visible to the threads that pass
-// bar.sync on the same barrier
-__device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
 // per-thread register budget of the executing warp group (all of its warps execute it): give registers back to the CTA's
 // pool / take them from it
@@ -106,11 +103,13 @@ __device__ __forceinline__ void wgmma_fence_operand(float (&d)[M]) {
 #pragma unroll
   for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// the same for the A fragments of register-A wgmmas (wgmma_tf32_ra): they must stay put until the batch has completed
-template <int M, int K>
+// the same for the A fragments of register-A wgmmas (wgmma_tf32_ra): they must stay put until the batch has completed.
+// R > 0: only rows [0, R) of `a`, the K steps a batch reads.
+template <int R = 0, int M, int K>
 __device__ __forceinline__ void wgmma_fence_operand(uint32_t (&a)[M][K]) {
+  static_assert(R <= M, "rows");
 #pragma unroll
-  for (int i = 0; i < M; ++i)
+  for (int i = 0; i < (R > 0 ? R : M); ++i)
 #pragma unroll
     for (int k = 0; k < K; ++k) asm volatile("" : "+r"(a[i][k])::"memory");
 }
