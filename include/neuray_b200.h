@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 6
+#define NR_ABI_VERSION 7
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -418,6 +418,22 @@ int nr_depth_loss(const NrDepthLossParams* p, void* stream);
  * prob0 (the rendered hit probability, a constant) and prob1 (hit_prob_self).  g == NULL: forward; otherwise d_prob1. */
 int nr_consistency_loss(const float* prob0, const float* prob1, int qn, int rn, int dn, float* loss, const float* g, float* d_prob1,
                         void* stream);
+
+/* ---- validation metrics ---------------------------------------------------------------------------------------- */
+
+#define NR_METRICS_MAX_PRED 8   /* predictions scored per nr_image_metrics call */
+
+/* PSNR_SSIM (reference network/metrics.py:13-79): the ground truth `gt` against each of `preds[0..n_pred)` (a HOST array of
+ * device pointers), all [h,w,3] fp32 in raster order.  Each image is quantised like color_map_backward (x*255 in fp32,
+ * clipped to [0,255], truncated) and cropped by margin_h rows top and bottom and margin_w columns left and right.
+ * out[n][4] (fp64) = the three per-channel sums of squared errors over the crop (exact integers) and the SSIM of
+ * skimage's structural_similarity(win_size=11, data_range=255): uniform 11x11 windows, sample covariance, the map less 5
+ * pixels on every side averaged per channel, then over the channels.  PSNR = 10 log10(255^2 / mse) with mse the mean of
+ * the three sse / ((h - 2 margin_h) (w - 2 margin_w)).  The result is the same bit for bit from run to run.  A crop
+ * smaller than 11 x 11 is NR_E_INVALID. */
+long long nr_image_metrics_workspace(int n_pred, int h, int w, int margin_h, int margin_w);   /* bytes */
+int nr_image_metrics(const float* gt, const float* const* preds, int n_pred, int h, int w, int margin_h, int margin_w, double* out,
+                     void* workspace, long long workspace_bytes, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------------------- */
 

@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -121,6 +121,8 @@ SIGNATURES = {
     "nr_render_loss": (C.c_int, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "nr_depth_loss": (C.c_int, [_vp, _vp]),
     "nr_consistency_loss": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "nr_image_metrics_workspace": (C.c_longlong, [_i, _i, _i, _i, _i]),
+    "nr_image_metrics": (C.c_int, [_vp, C.POINTER(_vp), _i, _i, _i, _i, _i, _vp, _vp, C.c_longlong, _vp]),
 }
 
 

@@ -12,8 +12,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libneuray_b200.so")
-SOURCES = ["nr_ops.cu", "nr_pack.cu", "nr_point_kernel.cu", "nr_ray_kernel.cu", "nr_tc_test.cu", "nr_train.cu", "nr_tape_gemm.cu", "nr_encoder.cu", "nr_losses.cu", "nr_mvs.cu"]
-HEADERS = ["nr_common.cuh", "nr_resample.cuh", "nr_tc.cuh", "nr_point_kernel_pm3.cuh", "nr_train_math.cuh", "nr_conv.cuh", "nr_loss_math.cuh", "nr_mvs.cuh", "nr_mvs_graph.cuh", "nr_encoder_graph.cuh", os.path.join("..", "..", "include", "neuray_b200.h")]
+SOURCES = ["nr_ops.cu", "nr_pack.cu", "nr_point_kernel.cu", "nr_ray_kernel.cu", "nr_tc_test.cu", "nr_train.cu", "nr_tape_gemm.cu", "nr_encoder.cu", "nr_losses.cu", "nr_mvs.cu", "nr_metrics.cu"]
+HEADERS = ["nr_common.cuh", "nr_resample.cuh", "nr_tc.cuh", "nr_point_kernel_pm3.cuh", "nr_train_math.cuh", "nr_conv.cuh", "nr_loss_math.cuh", "nr_mvs.cuh", "nr_mvs_graph.cuh", "nr_encoder_graph.cuh", "nr_metrics_math.cuh", os.path.join("..", "..", "include", "neuray_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]

@@ -13,6 +13,8 @@ What is rebound (SURVEY.md section 8b):
     DepthInitNet.forward / CostVolumeInitNet.forward -> neuray_b200.init_nets (inference: the whole init net natively, MVSNet included)
   * NeuralRayGenRenderer.predict_mean_for_depth_loss and network.loss.{RenderLoss, DepthLoss, ConsistencyLoss, name2loss}
     (SURVEY.md 8f row 3) -> neuray_b200.losses
+  * network.metrics.{PSNR_SSIM, name2metrics['psnr_ssim']} -> neuray_b200.metrics (the validation PSNR / SSIM on the GPU;
+    vis_img stays the reference's, it writes the JPEGs)
   * inference only: `render` runs image_encoder / vis_encoder natively into the frame pack (SURVEY.md 8f row 1,
     neuray_b200.encoders); with a gradient wanted through them the reference's own torch modules run
 Constructors, cfg keys, sub-module and state-dict names, and the output dict stay the reference's own.
@@ -21,7 +23,7 @@ kernels get a per-device table built by neuray_b200.weights.posenc_table.
 """
 import importlib
 
-from . import init_nets, init_ops, losses, render_ops, renderer
+from . import init_nets, init_ops, losses, metrics, render_ops, renderer
 
 _ORIGINALS = []          # (object, attribute name, original value) of everything install() rebound
 
@@ -71,6 +73,12 @@ def install():
             _rebind(ref_loss.name2loss, key, cls)
             _rebind(ref_loss, cls.__name__, cls)
     except Exception:      # a trimmed reference tree without the training code
+        pass
+    try:
+        ref_metrics = importlib.import_module("network.metrics")
+        _rebind(ref_metrics.name2metrics, "psnr_ssim", metrics.PSNR_SSIM)
+        _rebind(ref_metrics, "PSNR_SSIM", metrics.PSNR_SSIM)
+    except Exception:      # network.metrics needs skimage; a trimmed tree may not have it
         pass
     return base
 
