@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 7
+#define NR_ABI_VERSION 8
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -433,6 +433,32 @@ int nr_consistency_loss(const float* prob0, const float* prob1, int qn, int rn, 
  * smaller than 11 x 11 is NR_E_INVALID. */
 long long nr_image_metrics_workspace(int n_pred, int h, int w, int margin_h, int margin_w);   /* bytes */
 int nr_image_metrics(const float* gt, const float* const* preds, int n_pred, int h, int w, int margin_h, int margin_w, double* out,
+                     void* workspace, long long workspace_bytes, void* stream);
+
+/* Scores of the reference's eval.py for n pairs of uint8 [h,w,3] images in raster order, gt[n,h,w,3] against pr[n,h,w,3]
+ * (device pointers).  Each value is converted like color_map_forward, float(v) / 255 in fp32.
+ *
+ * nr_eval_metrics: out[n][2] (fp64) = tf.image.psnr(max_val 1) and tf.image.ssim(max_val 1, filter 11, sigma 1.5, k1 0.01,
+ * k2 0.03) of each pair, evaluated in fp64: PSNR = 10 log10(1 / mse) with mse over h*w*3 (inf for identical images); SSIM =
+ * the mean over the VALID (h-10) x (w-10) region and the channels of luminance * cs, from Gaussian-weighted means (window
+ * g (x) g, population covariance).  The result is the same bit for bit from run to run and for any n.  Images smaller than
+ * 11 x 11 are NR_E_INVALID. */
+long long nr_eval_metrics_workspace(int n, int h, int w);   /* bytes */
+int nr_eval_metrics(const uint8_t* gt, const uint8_t* pr, int n, int h, int w, double* out, void* workspace, long long workspace_bytes,
+                    void* stream);
+
+/* LPIPS-VGG (lpips.LPIPS(net='vgg'), version 0.1, called as eval.py calls it on x * 2 - 1): the scaling layer, torchvision's
+ * vgg16.features[0:30] with taps after relu1_2, relu2_2, relu3_3, relu4_3 and relu5_3, per tap each image's features divided
+ * by (their channel norm + 1e-10), the squared difference, the 1x1 lin weights and the spatial mean; out[n] (fp64) = the sum
+ * over the taps.  `params`: 31 tensors, features.{0,2,5,7,10,12,14,17,19,21,24,26,28}.weight and .bias in that order, then
+ * lin0..lin4.model.1.weight.  tf32x1 as for the encoders (0: 3xTF32, 1: one TF32 pass, what cuDNN runs under torch's
+ * default allow_tf32).  Images must be at least 32 x 32: a limit of this library, not of lpips (which takes 16 x 16), because
+ * nr_conv2d_nhwc needs conv5's input, h/16 x w/16, to be at least 2 x 2.  LPIPS of identical images is exactly 0.  The workspace
+ * grows with n (two [2n,h,w,64] fp32 buffers). */
+int nr_lpips_vgg_layout(int* n_tensors, long long* packed_floats);
+int nr_lpips_vgg_pack(const float* const* params, int n_params, float* packed, void* stream);
+long long nr_lpips_vgg_workspace(int n, int h, int w);   /* bytes */
+int nr_lpips_vgg_fwd(const float* packed, const uint8_t* gt, const uint8_t* pr, int n, int h, int w, double* out, int tf32x1,
                      void* workspace, long long workspace_bytes, void* stream);
 
 /* ---- diagnostics ------------------------------------------------------------------------------------------- */

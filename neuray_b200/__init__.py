@@ -8,6 +8,7 @@ Drop-in surface (SURVEY.md section 8b):
     neuray_b200.encoders        image_encoder (ResUNetLight) and vis_encoder, inference, channel-last into the frame pack
     neuray_b200.losses          predict_mean_for_depth_loss, RenderLoss / DepthLoss / ConsistencyLoss (forward + backward)
     neuray_b200.metrics         PSNR_SSIM, the validation PSNR / SSIM (network/metrics.py:13-79)
+    neuray_b200.eval_metrics    eval.py's scores: TensorFlow's PSNR / SSIM and LPIPS-VGG (python -m neuray_b200.eval scores a folder)
     neuray_b200.patch           installs them into an importable reference tree (render.py / run_training.py unchanged)
     neuray_b200.dist            ray-sharded rendering + gradient all-reduce over torch.distributed (NCCL)
 

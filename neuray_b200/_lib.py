@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -123,6 +123,12 @@ SIGNATURES = {
     "nr_consistency_loss": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "nr_image_metrics_workspace": (C.c_longlong, [_i, _i, _i, _i, _i]),
     "nr_image_metrics": (C.c_int, [_vp, C.POINTER(_vp), _i, _i, _i, _i, _i, _vp, _vp, C.c_longlong, _vp]),
+    "nr_eval_metrics_workspace": (C.c_longlong, [_i, _i, _i]),
+    "nr_eval_metrics": (C.c_int, [_vp, _vp, _i, _i, _i, _vp, _vp, C.c_longlong, _vp]),
+    "nr_lpips_vgg_layout": (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_longlong)]),
+    "nr_lpips_vgg_pack": (C.c_int, [_vp, _i, _vp, _vp]),
+    "nr_lpips_vgg_workspace": (C.c_longlong, [_i, _i, _i]),
+    "nr_lpips_vgg_fwd": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, C.c_longlong, _vp]),
 }
 
 
