@@ -11,29 +11,27 @@
 //     apart.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0 only, each from the
 //     whole row in the tile.
 //   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer, each layer as one 3xTF32 batch
-//     (mma_batch); both warp groups meet at a 256-thread barrier before a layer (its A columns come from both) and after
-//     the accumulator store (row_layer).  The dist-decoder
-//     heads (run_head) and the per-view tail base_fc.2 .. rgb_fc.0 (run_chain) are the exception: nothing in them is
-//     pooled or needs the row-owner layout, so each warp group runs them for its own 64 rows in the accumulator fragment
-//     (A from registers after the first layer, row sums over the 4 lanes that hold a row) and hands the results to the
-//     row owners through the tile and a small shared array (xch).  The ring's "empty" barriers count one arrival per
-//     compute warp group, so each releases those stages on its own.
+//     (mma_batch).  Every per-view layer runs in the accumulator fragment of the warp group that issues it, for its own
+//     64 rows: the dist-decoder heads (run_head), the front hit/vis .. base_fc.0 (in the kernel body) and the tail
+//     base_fc.2 .. rgb_fc.0 (run_chain).  Nothing in them is pooled or needs the row-owner layout; A comes from registers
+//     after each stretch's first layer, row sums run over the 4 lanes that hold a row, and the results go to the row
+//     owners through the tile and a small shared array (xch) at one 256-thread barrier per stretch.  The ring's "empty"
+//     barriers count one arrival per compute warp group, so each releases those stages on its own.
 //   * activation tile (80 KB of shared memory, 160 columns x 128 rows, tc::act_index): hi parts at columns [0,64), lo parts
 //     at [64,128), accumulator at [128,160).  base_fc.0 (N = 64) has its per-view inputs issued in two K rounds into one
-//     accumulator at [96,160): round A (the 32 neuray_feat inputs) right after prob_embed.2 while they are still the only
-//     live A operand, round B (the 40 rgb_feat inputs, lo parts at [48,88)) after ray_dir_fc.  Its epilogue reads the
-//     accumulator half by half, adds the point's view-pooled part and writes base_fc.2's operand over the columns it has
-//     already consumed (the same warp group owns column c and c + 32, so no other warp group reads them).  run_chain
-//     leaves x2 at [96,128) and rgb_fc.0's pre-activations at [128,144).
+//     accumulator, round A (the 32 neuray_feat inputs) and round B (the 40 rgb_feat inputs) with A from registers; the
+//     front stores it at [96,160).  Its epilogue reads the accumulator half by half, adds the point's view-pooled part and
+//     writes base_fc.2's operand over the columns it has already consumed (the same warp group owns column c and c + 32,
+//     so no other warp group reads them).  run_chain leaves x2 at [96,128) and rgb_fc.0's pre-activations at [128,144).
 //   * per-point layers: the view-pooled part of base_fc.0 (K 140 -> 160) and geometry_fc.0 have the same inputs for every
 //     view of a point, so they are multiplied once per point, not once per row: the pooled statistics go into a compact
-//     operand of PB rows (one per point, in tile columns [0,96) while those are dead), the eight compute warps multiply
+//     operand of PB rows (one per point, in tile columns [0,64) while those are dead), the eight compute warps multiply
 //     it with warp-level mma.sync (3xTF32, B read straight from the weight ring stages, warp w computes outputs
 //     8w .. 8w + 7) into a [PB][64] result in shared memory (OFF_PT), and every row of the point reads it from there.
 //   * the rest of shared memory: 4 x 16 KB weight ring (TMA bulk copies, fed by the producer group; the view-pooled
 //     base_fc.0 weights stream through it as five more stages), the resident tile of ray_dir_fc.2, small weights, camera
 //     blocks, the row-scalar exchange, the per-point result, and one [32][36] transposition buffer per warp: gather (16
-//     channels per warp group in two passes: ray_feats, then img_feats, which stay there until ray_dir_fc needs them), the
+//     channels per warp group in two passes: ray_feats, then img_feats, which stay there until rgb_feat is built), the
 //     cross-view pooling (pm::pool_rows) and the lane-group sums of the non-power-of-two groups all go through it.
 #pragma once
 
@@ -60,7 +58,8 @@ constexpr int NTHR = NCOMP + 128;                             // + a producer wa
 // compute groups take them: 128 x 24 + 256 x 240 = 64512 of the SM's 65536
 constexpr int REG_PROD = 24, REG_COMP = 240;
 static_assert(128 * REG_PROD + NCOMP * REG_COMP <= 65536, "register file");
-constexpr int BAR_LAYER = 1;                                  // named barrier of the compute warp groups: around every layer
+constexpr int BAR_LAYER = 1;                                  // named barrier of both compute warp groups
+constexpr int BAR_WG = 2;                                     // + wg: named barrier of one compute warp group's 128 threads
 constexpr int TCOLS = 160;                                    // activation-tile columns
 constexpr int ACT = (TCOLS / 32) * 4096;                      // floats per activation tile
 
@@ -75,8 +74,11 @@ constexpr int OFF_STG = OFF_SW + SW;                          // gather transpos
 constexpr int STG_ROW = 36;
 constexpr int STG = (NCOMP / 32) * 32 * STG_ROW;
 constexpr int OFF_XCH = OFF_STG + STG;                        // row scalars handed between the warp groups: [slot][128 rows], slots XCH_*
-// (o0, o1) of the 4 heads; once the heads' outputs are read, the chain's row scalars w1, mrow, dd[0..3] | vis_fc2 visibility
-constexpr int XCH_HEAD = 0, XCH_ROW = 0, XCH_L2 = 8, XCH = 9 * 128;
+// (o0, o1) of the 4 heads | the row scalars zrow, ihp, ihc, mrow, dd[0..3], rgbin[0..2] (XCH_FRONT + k, written before the
+// heads; mrow, dd and rgbin stay there for the chain and the colour blend).  Once a warp group has read its rows' head
+// outputs, the front's outputs over them: the neuray_fc gate and rgb_feat columns 32..34.  After pooling #1 the chain's
+// w1 over the gate, and its vis_fc2 visibility over zrow.
+constexpr int XCH_HEAD = 0, XCH_FRONT = 8, XCH_GATE = 0, XCH_RF = 1, XCH_W1 = 0, XCH_L2 = 8, XCH = 19 * 128;
 constexpr int OFF_PT = OFF_XCH + XCH;                         // per-point layer outputs: [point][PT_ROW] (64 used), at most 32 points
 constexpr int PT_ROW = 72;
 constexpr int PT = 32 * PT_ROW;
@@ -90,10 +92,19 @@ static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 static_assert(OFF_STAB % 4 == 0, "alignment");
 static_assert((OFF_ACT * 4) % 1024 == 0 && (OFF_RD1 * 4) % 1024 == 0 && OFF_WG1 % 4 == 0 && OFF_SW % 4 == 0 && OFF_STG % 4 == 0 &&
                   OFF_PT % 4 == 0, "alignment");
-// the per-point operand of a per-point layer: [point][OP_ROW] (K 160 used) in activation-tile columns [0,96), which are
-// dead while it is used (after base_fc.0's round B until its epilogue; after rgb_fc.0 until the next tile's gather)
+// the per-point operand of a per-point layer: [point][OP_ROW] (K 160 used) in the first two slabs of the activation tile
+// (columns [0,64)), which are dead while it is used (after base_fc.0's round B until its epilogue; after rgb_fc.0 until the
+// next tile's gather).  Pooling #1 reads rgb_feat from the third slab (columns [64,96)) while its operand fills up.
 constexpr int OP_ROW = 164;                                   // = 4 mod 32: the 32 lanes of an A-fragment load hit 32 banks
-static_assert(32 * OP_ROW <= 3 * 4096, "per-point operand");
+static_assert(32 * OP_ROW <= 2 * 4096, "per-point operand");
+// rgb_feat columns 0..31 on their way from the front to pooling #1, in fp32, in tile slab 2 (columns [64,96)): row r,
+// column c at RF_SLAB + rf_slab_index(r, c).  Rows 64c .. 64c + 63 keep to the half of the slab that holds those rows in
+// the tile's own layout (floats 2048c .. 2048c + 2047), so the front of warp group c writes only its own rows: the other
+// warp group may still be reading its half of the slab (ray_feats' lo part, A of its heads and of its prob_embed.0).
+constexpr int RF_SLAB = 2 * 4096;
+__host__ __device__ constexpr int rf_slab_index(int r, int c) { return (r >> 6) * 2048 + (c >> 2) * 256 + (r & 63) * 4 + (c & 3); }
+static_assert(rf_slab_index(63, 31) < 2048 && rf_slab_index(64, 0) == 2048 && rf_slab_index(127, 31) < 4096 &&
+                  tc::act_index(64, 64) - RF_SLAB == 2048, "rgb_feat: each warp group's rows in its own half of slab 2");
 
 // ---- per-point layers: [points x K] x [K x 64] on warp-level mma.sync, 3xTF32 ----
 // Compute warp w (of 8) computes outputs 8w .. 8w + 7 for all PB points of the tile: MT m16 tiles of points, and one
@@ -214,42 +225,33 @@ __device__ __forceinline__ void mma_batch(float (&d)[N / 2], const A& a, const B
   a.template pin<KS>();
 }
 
-// A row-owner layer, executed by both compute warp groups after they wrote their A columns; warp group c multiplies rows
-// 64c .. 64c + 63.  b_ready() runs once both are at the layer: it waits for the B operand's ring stages, if any, and
-// returns its descriptors.  ACC: onto what the accumulator columns [DCOL, DCOL + N) hold.  Returns with the outputs in
-// those columns, visible to every row owner of both warp groups, and both warp groups' reads of B completed.
-template <int N, int KS, int DCOL, bool ACC, class BReady>
-__device__ __forceinline__ void row_layer(const Blk& b, const TileA& a, BReady&& b_ready) {
-  tc::fence_proxy_async_smem();              // this thread's A columns -> visible to the tensor cores
-  tc::named_sync(BAR_LAYER, NCOMP);
-  const auto bd = b_ready();
-  float d[N / 2];
-  if (ACC) tc::acc_load_half<N>(b.act, DCOL, b.row, b.wg, d);
-  mma_batch<N, KS, ACC>(d, a, bd, [] {});
-  tc::acc_store_half<N>(b.act, DCOL, b.row, b.wg, d);
-  tc::named_sync(BAR_LAYER, NCOMP);
-}
-
-// ---- layers in the accumulator fragment of the warp group that issues them (the heads and the per-view chain) ----
+// ---- layers in the accumulator fragment of the warp group that issues them (the heads, the front and the chain) ----
 // This thread holds columns 8j + 2q + {0, 1} of fragment rows fr and fr + 8 (q = t % 4, tc::acc_load_half):
 // d[4j + 2r + e] is column 8j + 2q + e of row fr + 8r.
+// An A fragment (tc::wgmma_tf32_ra) wants columns 8j + q and 8j + q + 4 of rows fr, fr + 8 instead.  frag_cols turns one
+// row's pair of group j (x0, x1 = columns 8j + 2q, 8j + 2q + 1) into those two columns (c0 = 8j + q, c4 = 8j + q + 4):
+// lane q of a quad reads lane s = 2 (q & 1) + (q >> 1) in the first shuffle and lane s ^ 2 in the second; a lane offers
+// column 2q + (q >> 1) in the first and its other column in the second, and what arrives is column q and q + 4 (in that
+// order for even q, swapped for odd q).
+__device__ __forceinline__ void frag_cols(float x0, float x1, int lane, float& c0, float& c4) {
+  const int q = lane & 3, s1 = (lane & ~3) | ((q & 1) << 1) | (q >> 1);
+  const float r1 = __shfl_sync(0xffffffffu, q >> 1 ? x1 : x0, s1);
+  const float r2 = __shfl_sync(0xffffffffu, q >> 1 ? x0 : x1, s1 ^ 2);
+  c0 = q & 1 ? r2 : r1;
+  c4 = q & 1 ? r1 : r2;
+}
 // An N = 32 fragment x (after its epilogue) -> the A fragments of the next layer's 4 K steps, split into hi / lo
-// (ah[j], al[j], j < 4).  A K step wants columns 8j + q and 8j + q + 4 of rows fr, fr + 8 (tc::wgmma_tf32_ra): lane q of
-// a quad reads lane s = 2 (q & 1) + (q >> 1) in the first shuffle and lane s ^ 2 in the second; a lane offers column
-// 2q + (q >> 1) in the first and its other column in the second, and what arrives is column q and q + 4 (in that order
-// for even q, swapped for odd q).
+// (ah[j], al[j], j < 4)
 template <int KA>
 __device__ __forceinline__ void frag_to_a(const float (&x)[16], int lane, uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4]) {
-  const int q = lane & 3, s1 = (lane & ~3) | ((q & 1) << 1) | (q >> 1);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float x0 = x[4 * j + 2 * r], x1 = x[4 * j + 2 * r + 1];
-      const float r1 = __shfl_sync(0xffffffffu, q >> 1 ? x1 : x0, s1);
-      const float r2 = __shfl_sync(0xffffffffu, q >> 1 ? x0 : x1, s1 ^ 2);
-      tc::split_tf32(q & 1 ? r2 : r1, ah[j][r], al[j][r]);              // column 8j + q of row fr + 8r
-      tc::split_tf32(q & 1 ? r1 : r2, ah[j][2 + r], al[j][2 + r]);      // column 8j + q + 4
+      float c0, c4;
+      frag_cols(x[4 * j + 2 * r], x[4 * j + 2 * r + 1], lane, c0, c4);
+      tc::split_tf32(c0, ah[j][r], al[j][r]);                          // column 8j + q of row fr + 8r
+      tc::split_tf32(c4, ah[j][2 + r], al[j][2 + r]);                  // column 8j + q + 4
     }
   }
 }
@@ -267,6 +269,18 @@ __device__ __forceinline__ void row_dot(const float (&z)[16], const float* __res
 #pragma unroll
         for (int r = 0; r < 2; ++r) s[r] = fmaf(w[8 * j + 2 * qs + e], __shfl_sync(0xffffffffu, z[4 * j + 2 * r + e], (lane & ~3) | qs), s[r]);
       }
+    }
+  }
+}
+// the same over one 8-column group: z[2r + e] is its column 2q + e of row fr + 8r
+__device__ __forceinline__ void row_dot8(const float (&z)[4], const float* __restrict__ w, float bias, int lane, float (&s)[2]) {
+  s[0] = s[1] = bias;
+#pragma unroll
+  for (int qs = 0; qs < 4; ++qs) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) s[r] = fmaf(w[2 * qs + e], __shfl_sync(0xffffffffu, z[2 * r + e], (lane & ~3) | qs), s[r]);
     }
   }
 }
@@ -322,7 +336,7 @@ __device__ __forceinline__ void run_head(const Blk& b, Ring& ring, const float* 
 // The per-view tail base_fc.2 -> vis_fc.0 -> vis_fc.2 -> vis_fc2.0 -> rgb_fc.0 for the 64 rows whose MMAs this warp
 // group issues, in its accumulator fragment and without meeting the other warp group: nothing in it pools across views.
 // base_fc.2 reads its A (K 64) from the tile, where both warp groups' row owners wrote it before the barrier in front of
-// the chain, together with the row scalars w1, mrow and dd[0..3] in xch slots XCH_ROW + [0,6); every later layer takes
+// the chain, together with w1 in xch slot XCH_W1 (mrow and dd[0..3] are still in XCH_FRONT + 3 .. 7); every later layer takes
 // A from registers.  vis_fc.1 and vis_fc2.1 are summed by the quad that holds a row, in column order (row_dot), so every
 // value is bit-identical to a round trip through the row owners.  Leaves x2 (base_fc.2's output +
 // the vis_fc residual) in tile columns [96,128), rgb_fc.0's pre-activations in [128,144) and vis2 in xch slot XCH_L2.
@@ -338,11 +352,11 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
   mma_batch<32, 8>(d, tile_a(b, 0, 64), tile_b(w, tcl::B1_L), [&] {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float* __restrict__ x = xch + XCH_ROW * 128 + fr + 8 * r;
-      w1[r] = x[0];
-      mr[r] = x[128];
-      t0[r] = q == 0 ? 0.f : x[(1 + q) * 128];
-      t1[r] = q == 0 ? x[5 * 128] : 0.f;
+      const float* __restrict__ x = xch + XCH_FRONT * 128 + fr + 8 * r;
+      w1[r] = xch[XCH_W1 * 128 + fr + 8 * r];
+      mr[r] = x[3 * 128];
+      t0[r] = q == 0 ? 0.f : x[(3 + q) * 128];
+      t1[r] = q == 0 ? x[7 * 128] : 0.f;
     }
   });
   ring.release(0);
@@ -430,6 +444,13 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
   ring.release(2);
   ring.advance(3);
   tc::acc_store_half<16>(b.act, 128, b.row, b.wg, g);
+}
+
+// x as a value the compiler cannot see through: what is computed from it is not hoisted out of a loop
+__device__ __forceinline__ int opaque(int x) {
+  int y;
+  asm volatile("mov.b32 %0, %1;" : "=r"(y) : "r"(x));
+  return y;
 }
 
 // ---- this thread's columns of its row ----
@@ -767,7 +788,24 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         for (int k = 0; k < 16; ++k) o[12 + 8 * (k >> 2) + 4 * wg + (k & 3)] = x[k];
       }
     }
-    gather16(32);                                                                  // img_feats: stay in the buffer until ray_dir_fc
+    gather16(32);                                                                  // img_feats: stay in the buffer until rgb_feat is built
+    {
+      // the row scalars of the front's fragment rows, read after the heads: zrow, ihp, ihc, mrow, dd[0..1] from warp
+      // group 0, dd[2..3], rgbin[0..2] from warp group 1
+      const float rs[11] = {zrow, ihp, ihc, mrow, dd[0], dd[1], dd[2], dd[3], rgbin[0], rgbin[1], rgbin[2]};
+#pragma unroll
+      for (int k = 0; k < 5; ++k) xch[(XCH_FRONT + 6 * wg + k) * 128 + row] = wg ? rs[6 + k] : rs[k];
+      if (wg == 0) xch[(XCH_FRONT + 5) * 128 + row] = rs[5];
+    }
+    if (DEBUG && kp.dbg != nullptr && row_ok) {                                   // the row scalars and img_feats (hit, vis: in the front)
+      float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
+      const float* __restrict__ mine = stg + lane * STG_ROW;
+      for (int k = 0; k < 16; ++k) o[44 + 8 * (k >> 2) + 4 * wg + (k & 3)] = mine[k];
+      if (wg == 0) {
+        o[0] = mrow; o[1] = zrow; o[4] = dbg_px; o[5] = dbg_py;
+        o[6] = dbg_dir[0]; o[7] = dbg_dir[1]; o[8] = dbg_dir[2]; o[9] = rgbin[0]; o[10] = rgbin[1]; o[11] = rgbin[2];
+      }
+    }
     PM_TICK(3)
     // the heads: each warp group runs them for the 64 rows whose MMAs it issues (run_head); A[0:32] comes from both
     tc::fence_proxy_async_smem();
@@ -775,135 +813,214 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #pragma unroll 1
     for (int hd = 0; hd < n_heads; ++hd) run_head(b, ring, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
     PM_TICK(4)
-    tc::named_sync(BAR_LAYER, NCOMP);                                              // head outputs -> the row owners
-    // hit and visibility go into warp group 0's columns
-    float hit = 0.f, visib = 0.f;
-    if (wg == 0) {
-      float hv[4][2];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        hv[k][0] = k < n_heads ? xch[(XCH_HEAD + 2 * k) * 128 + row] : 0.f;
-        hv[k][1] = k < n_heads ? xch[(XCH_HEAD + 2 * k + 1) * 128 + row] : 0.f;
-      }
-      const float* vp = smem + OFF_CAM + 32 + (v < rfn ? v : 0) * 20;
-      const float zc = fmaxf(zrow, 1e-5f);
-      const float a = vp[15], bb = vp[16];
-      const float tz = (-1.f / zc - a) / (bb - a);
-      const float lo = tz - ihp, hi = tz + ihc;
-      const float aw = sigmoidf_(hv[2][0]);
-      const float vd = pp.use_vis ? sigmoidf_(hv[3][0]) : 1.f;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const float mean = softplusf_(hv[0][i]);
-        const float var = softplusf_(hv[1][i]) + pp.var_bias;
-        const float c0 = logistic_cdf((lo - mean) * var) * vd, c1 = logistic_cdf((hi - mean) * var) * vd;
-        const float mix = i == 0 ? aw : 1.f - aw;
-        visib = fmaf(1.f - c0, mix, visib);
-        hit = fmaf(c1 - c0, mix, hit);
-      }
-      visib *= mrow; hit *= mrow;
-    }
 
-    // ---------------- prob_embed (tensor cores), neuray_fc, ray_dir_fc ----------------
+    // ---------------- the front, hit/vis through base_fc.0: each warp group for its own 64 rows, in its accumulator fragment ----------------
+    // Nothing in it pools across views, so it needs no barrier with the other warp group until its outputs go to the row
+    // owners: every shared-memory write in it lands in this warp group's own rows (of the tile, RF_SLAB and xch), which
+    // only it reads before the hand-off barrier.  Every accumulator gets the products and every row sum the order the row owners gave them, so every value
+    // is bit-identical to a round trip through them.  Ring stages (each warp group waits and releases on its own):
+    // prob_embed.0 (tcl::PE0_L) | prob_embed.2 + neuray_fc.0 (tcl::PE1_L) | base_fc.0 x3 (tcl::B0_L); ray_dir_fc.2 is resident.
     {
-      float x[4] = {0.f, 0.f, 0.f, 0.f};
-      if (wg == 0) { x[0] = (hit - 0.5f) * 2.f; x[1] = (visib - 0.5f) * 2.f; }
-      st_own<1>(b, 32, 96, x);                                                     // A[32:40] = hit', vis', 0... (the heads' hidden layer is dead)
-    }
-    // prob_embed.0: K = 32 + 8, accumulator columns [128,160)
-    row_layer<32, 5, 128, false>(b, tile_a(b, 0, 64), [&] { return tile_b(ring.wait(0).addr, tcl::PE0_L); });
-    ring.release(0);
-    ring.advance(1);
-    {
-      float x[16];
-      ld_own<4>(b, 128, x);
-      add_bias_own<4>(b, x, sw + SW_PE0B);
+      // fr_f, lane_f: fr and the lane as values the compiler cannot see through.  The front's per-thread addresses are
+      // then worked out here in every tile instead of being hoisted out of the tile loop and held in registers across the
+      // chain (which made the DEBUG instantiations spill).  In the comments below, fr stands for fr_f.
+      const int fr_f = opaque(fr), lane_f = opaque(lane);
+      const int q = lane_f & 3;
+      const float* __restrict__ xf = xch + XCH_FRONT * 128;                       // xf[k * 128 + r]: row scalar k of row r
+      // hit and visibility of row fr + 8 (q >> 1) (lanes q and q ^ 1 both compute it) from its heads' outputs
+      float hv01;                                                                  // hit' (even q) or vis' (odd q)
+      {
+        const int rr = fr_f + 8 * (q >> 1);
+        __syncwarp();                                                              // run_head: this warp's lanes wrote rows fr, fr + 8
+        float hv[4][2];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) x[j] = fmaxf(x[j], 0.f);
-      st_own<4>(b, 0, 64, x);                                                      // over ray_feats: their last reader has completed
-    }
-    PM_TICK(5)
-    // prob_embed.2 with neuray_fc.0 behind it: N = 48, accumulator columns [96,144)
-    row_layer<48, 4, 96, false>(b, tile_a(b, 0, 64), [&] { return tile_b(ring.wait(0).addr, tcl::PE1_L); });
-    ring.release(0);
-    ring.advance(1);
-    float gate;
-    {
-      float x[16];
-      ld_own<4>(b, 96, x);
-      add_bias_own<4>(b, x, sw + SW_PE1B);                                         // neuray_feat
-      st_own<4>(b, 0, 64, x);
-      float h8[8];
-      ld_row<2>(b, 128, h8);                                                       // neuray_fc.0 pre-activations (both warp groups: the whole row)
-      gate = sw[SW_NF1B];
+        for (int k = 0; k < 4; ++k) {
+          hv[k][0] = k < n_heads ? xch[(XCH_HEAD + 2 * k) * 128 + rr] : 0.f;
+          hv[k][1] = k < n_heads ? xch[(XCH_HEAD + 2 * k + 1) * 128 + rr] : 0.f;
+        }
+        // (point, view) of row rr, as the row owners get theirs
+        const int l = rr & 31, g = l / G;
+        const int rv = P2 ? l % G : l - g * G;
+        const float* vp = smem + OFF_CAM + 32 + (rv < rfn ? rv : 0) * 20;
+        const float zc = fmaxf(xf[rr], 1e-5f);
+        const float a = vp[15], bb = vp[16];
+        const float tz = (-1.f / zc - a) / (bb - a);
+        const float lo = tz - xf[128 + rr], hi = tz + xf[2 * 128 + rr];
+        const float aw = sigmoidf_(hv[2][0]);
+        const float vd = pp.use_vis ? sigmoidf_(hv[3][0]) : 1.f;
+        float hit = 0.f, visib = 0.f;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) gate = fmaf(sw[SW_NF1W + j], elu(h8[j] + sw[SW_NF0C + j]), gate);
-    }
-    // base_fc.0, K round A: the neuray_feat inputs (its K steps 5..8), accumulator columns [96,160); waits for all three
-    // of its stages, which round B reads too
-    row_layer<64, 4, 96, false>(b, tile_a(b, 0, 64), [&] {
+        for (int i = 0; i < 2; ++i) {
+          const float mean = softplusf_(hv[0][i]);
+          const float var = softplusf_(hv[1][i]) + pp.var_bias;
+          const float c0 = logistic_cdf((lo - mean) * var) * vd, c1 = logistic_cdf((hi - mean) * var) * vd;
+          const float mix = i == 0 ? aw : 1.f - aw;
+          visib = fmaf(1.f - c0, mix, visib);
+          hit = fmaf(c1 - c0, mix, hit);
+        }
+        const float mr = xf[3 * 128 + rr];
+        visib *= mr; hit *= mr;
+        if (DEBUG && kp.dbg != nullptr && (q & 1) == 0) {
+          const int rn_ = n - pl + (P2 ? rr / G : (rr >> 5) * PPW + g);            // n - pl: the block's first point
+          if ((P2 ? rn_ < N : (rn_ < N && g < PPW)) && rv < rfn) {
+            float* __restrict__ o = kp.dbg + (size_t(rv) * N + rn_) * 76;
+            o[2] = hit; o[3] = visib;
+          }
+        }
+        hv01 = q & 1 ? (visib - 0.5f) * 2.f : (hit - 0.5f) * 2.f;
+      }
+      // prob_embed.0's K step 4 of rows fr, fr + 8 (columns 32, 33 = hit', vis', the rest 0) -> this warp group's rows of
+      // the tile (the heads' hidden layer is dead); lanes 0 and 1 have their row fr values, lanes 2 and 3 the row fr + 8 ones
+      {
+        const float other = __shfl_xor_sync(0xffffffffu, hv01, 2);
+        uint32_t* const at = reinterpret_cast<uint32_t*>(b.act);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          uint32_t h, l;
+          tc::split_tf32(q < 2 ? (r ? other : hv01) : 0.f, h, l);
+          const int rr = fr_f + 8 * r;
+          at[tc::act_index(rr, 32 + q)] = h;
+          at[tc::act_index(rr, 96 + q)] = l;
+          at[tc::act_index(rr, 36 + q)] = 0u;
+          at[tc::act_index(rr, 100 + q)] = 0u;
+        }
+      }
+      tc::fence_proxy_async_smem();
+      tc::named_sync(BAR_WG + wg, 128);
+      // prob_embed.0: K = 32 + 8 (ray_feats, hit' and vis'), A from the tile; ReLU, then into prob_embed.2's A layout
+      uint32_t ah[4][4], al[4][4];
+      {
+        float d[16];
+        mma_batch<32, 5>(d, tile_a(b, 0, 64), tile_b(ring.wait(0).addr, tcl::PE0_L), [] {});
+        ring.release(0);
+        ring.advance(1);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 bb = *reinterpret_cast<const float2*>(sw + SW_PE0B + 8 * j + 2 * q);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            d[4 * j + 2 * r] = fmaxf(d[4 * j + 2 * r] + bb.x, 0.f);
+            d[4 * j + 2 * r + 1] = fmaxf(d[4 * j + 2 * r + 1] + bb.y, 0.f);
+          }
+        }
+        frag_to_a(d, lane_f, ah, al);
+      }
+      PM_TICK(5)
+      // prob_embed.2 with neuray_fc.0 behind it (N = 48): neuray_feat = columns [0,32) + bias, the gate from columns [32,40)
+      float gate[2];
+      {
+        float d[24];
+        mma_batch<48, 4>(d, RegA<4>{ah, al}, tile_b(ring.wait(0).addr, tcl::PE1_L), [] {});
+        ring.release(0);
+        ring.advance(1);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 bb = *reinterpret_cast<const float2*>(sw + SW_PE1B + 8 * j + 2 * q);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            d[4 * j + 2 * r] += bb.x;
+            d[4 * j + 2 * r + 1] += bb.y;
+          }
+        }
+        // neuray_fc.0's ELU in the lane that holds the column, neuray_fc.1 over the quad in column order
+        float y[4];
+        const float2 c = *reinterpret_cast<const float2*>(sw + SW_NF0C + 2 * q);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          y[2 * r] = elu(d[16 + 2 * r] + c.x);
+          y[2 * r + 1] = elu(d[16 + 2 * r + 1] + c.y);
+        }
+        row_dot8(y, sw + SW_NF1W, sw[SW_NF1B], lane_f, gate);
+        float nf[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) nf[j] = d[j];
+        frag_to_a(nf, lane_f, ah, al);
+      }
+      // base_fc.0, K round A: the neuray_feat inputs (its K steps 5..8).  Waits for all three of its stages, which round B
+      // reads too.  Under its MMAs: the gate goes to the row owners' slot, and ray_dir_fc.0 (K 4, N 16) runs on the CUDA
+      // cores straight into ray_dir_fc.2's A fragments (column u = hidden unit u)
       ring.wait(0);
       ring.wait(1);
       ring.wait(2);
-      return base0_b(ring, 5);
-    });
-    // rgb_feat (35) + zero padding: rf[4q + i] = column 8q + 4wg + i
-    float rf[20];
-    {
-      {
-        float h8[8];
+      float acc[32];
+      uint32_t rh[2][4], rl[2][4];
+      mma_batch<64, 4>(acc, RegA<4>{ah, al}, base0_b(ring, 5), [&] {
+        if (q < 2) xch[XCH_GATE * 128 + fr_f + 8 * q] = q ? gate[1] : gate[0];
         const float* __restrict__ w0 = sw + SW_RD0W;
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const float4 b4 = own4(b, sw + SW_RD0B, q), k0 = own4(b, w0, q), k1 = own4(b, w0 + 16, q), k2 = own4(b, w0 + 32, q), k3 = own4(b, w0 + 48, q);
-          h8[4 * q] = elu(fmaf(k3.x, dd[3], fmaf(k2.x, dd[2], fmaf(k1.x, dd[1], fmaf(k0.x, dd[0], b4.x)))));
-          h8[4 * q + 1] = elu(fmaf(k3.y, dd[3], fmaf(k2.y, dd[2], fmaf(k1.y, dd[1], fmaf(k0.y, dd[0], b4.y)))));
-          h8[4 * q + 2] = elu(fmaf(k3.z, dd[3], fmaf(k2.z, dd[2], fmaf(k1.z, dd[1], fmaf(k0.z, dd[0], b4.z)))));
-          h8[4 * q + 3] = elu(fmaf(k3.w, dd[3], fmaf(k2.w, dd[2], fmaf(k1.w, dd[1], fmaf(k0.w, dd[0], b4.w)))));
-        }
-        st_own<2>(b, 48, 64, h8);                                                  // ray_dir_fc.2 operand: hi [48,64), lo [64,80)
-      }
-      // ray_dir_fc.2: K = 16, accumulator [0,48)
-      row_layer<48, 2, 0, false>(b, tile_a(b, 48, 16), [&] { return tile_b(tc::smem_u32(smem + OFF_RD1), tcl::RD1_L); });
-      ld_own<5>(b, 0, rf);
-      // + [rgb | img_feats]: column c holds img_feats channel c - 3, which warp group ((c - 3) >> 2) & 1 gathered into
-      // its buffer column 4 ((c - 3) >> 3) + ((c - 3) & 3).  Of this warp group's columns 8q + 4wg + i, i = 3 is in its own
-      // buffer (column 4q), i < 3 in the other warp group's (column 4(q - 1 + wg) + 1 + i).
-      const float* __restrict__ mine = stg + lane * STG_ROW;
-      const float* __restrict__ other = smem + OFF_STG + (warp ^ 4) * 32 * STG_ROW + lane * STG_ROW;
+        for (int r = 0; r < 2; ++r) {
+          const int rr = fr_f + 8 * r;
+          const float d0 = xf[4 * 128 + rr], d1 = xf[5 * 128 + rr], d2 = xf[6 * 128 + rr], d3 = xf[7 * 128 + rr];
 #pragma unroll
-      for (int q = 0; q < 5; ++q) {
-        const float4 bb = own4(b, sw + SW_RD1B, q);                                // (q = 4, wg = 1: past the 36 biases, unused)
-        float* r = rf + 4 * q;
-        r[0] = elu(r[0] + bb.x); r[1] = elu(r[1] + bb.y); r[2] = elu(r[2] + bb.z); r[3] = elu(r[3] + bb.w);
-        if (q == 0 && wg == 0) {
-          r[0] += rgbin[0]; r[1] += rgbin[1]; r[2] += rgbin[2];
-        } else if (q < 4 || wg == 0) {
+          for (int s = 0; s < 2; ++s) {
 #pragma unroll
-          for (int i = 0; i < 3; ++i) r[i] += other[4 * (q - 1 + wg) + 1 + i];
+            for (int h = 0; h < 2; ++h) {
+              const int u = 8 * s + 4 * h + q;
+              const float x = elu(fmaf(w0[48 + u], d3, fmaf(w0[32 + u], d2, fmaf(w0[16 + u], d1, fmaf(w0[u], d0, sw[SW_RD0B + u])))));
+              tc::split_tf32(x, rh[s][2 * h + r], rl[s][2 * h + r]);
+            }
+          }
         }
-        if (q < 4) r[3] += mine[4 * q];
-        if (q == 4) {
-          if (wg == 0) r[3] = 1.f;                                                 // constant input: base_fc.0's bias is column 35 of its tile
-          else r[0] = r[1] = r[2] = r[3] = 0.f;
+      });
+      // ray_dir_fc.2: K = 16, N = 48 (35 used)
+      float e[24];
+      mma_batch<48, 2>(e, RegA<2>{rh, rl}, tile_b(tc::smem_u32(smem + OFF_RD1), tcl::RD1_L), [] {});
+      // rgb_feat (35) + the constant 1 (column 35: base_fc.0's bias) + zero padding, in round B's A fragments.  Column c < 35
+      // is elu(ray_dir_fc.2 + bias) + rgbin[c] (c < 3) or img_feats channel c - 3, which warp group ((c - 3) >> 2) & 1
+      // gathered into its buffer column 4 ((c - 3) >> 3) + ((c - 3) & 3), row rr at lane rr & 31 of its warp rr >> 5.
+      // Columns < 35 also go to the row owners in fp32 for pooling #1: [0,32) to tile slab 2 (RF_SLAB), [32,35) to xch.
+      // Of K step s, column 8s + 4h + q: img_feats channel 8s + 4h + q - 3 of row fr is at im[h] + 4s (h = 0: own buffer
+      // for q = 3, the other's column 4 (s - 1) + q + 1 for q < 3; h = 1: own buffer column 4s + q + 1 for q < 3, the
+      // other's column 4s for q = 3); row fr + 8 is 8 buffer rows further.
+      uint32_t bh[5][4], bl[5][4];
+      {
+        const float* __restrict__ img0 = smem + OFF_STG + ((fr_f >> 5) * 32 + (fr_f & 31)) * STG_ROW;
+        const float* __restrict__ img1 = img0 + 4 * 32 * STG_ROW;
+        const float* __restrict__ im[2] = {q == 3 ? img0 : img1 + q - 3, q < 3 ? img0 + q + 1 : img1};
+        float* __restrict__ rfo = b.act + RF_SLAB + rf_slab_index(fr_f, q);          // column 8s + 4h + q of row fr + 8r: rfo[(2s + h) * 256 + 32r]
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+#pragma unroll
+          for (int s = 0; s < 5; ++s) {
+            float x[2];
+            frag_cols(e[4 * s + 2 * r], e[4 * s + 2 * r + 1], lane_f, x[0], x[1]);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int c = 8 * s + 4 * h + q;
+              float f = c == 35 ? 1.f : 0.f;
+              if (c < 35) {
+                f = elu(x[h] + sw[SW_RD1B + c]);
+                if (c < 3) f += xf[(8 + q) * 128 + fr_f + 8 * r];
+                else f += im[h][4 * s + 8 * r * STG_ROW];
+                if (s < 4) rfo[(2 * s + h) * 256 + 32 * r] = f;
+                else xch[(XCH_RF + q) * 128 + fr_f + 8 * r] = f;
+              }
+              tc::split_tf32(f, bh[s][2 * h + r], bl[s][2 * h + r]);
+            }
+          }
         }
       }
-      if (DEBUG && kp.dbg != nullptr && row_ok) {
-        float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
-        for (int k = 0; k < 16; ++k) o[44 + 8 * (k >> 2) + 4 * wg + (k & 3)] = mine[k];
-      }
-      st_own<5>(b, 0, 48, rf);                                                     // rgb_feat: hi [0,40), lo [48,88)
+      // base_fc.0, K round B: rgb_feat (its K steps 0..4), onto round A's accumulators
+      mma_batch<64, 5, true>(acc, RegA<5>{bh, bl}, base0_b(ring, 0), [] {});
+#pragma unroll
+      for (int s = 0; s < 3; ++s) ring.release(s);
+      ring.advance(3);
+      tc::acc_store_half<64>(b.act, 96, b.row, b.wg, acc);
     }
-    // base_fc.0, K round B: rgb_feat (its K steps 0..4), onto round A's accumulators
-    row_layer<64, 5, 96, true>(b, tile_a(b, 0, 48), [&] { return base0_b(ring, 0); });
+    // Hand-off to the row owners.  Live in the tile: base_fc.0's per-view accumulator (bias included) in columns [96,160)
+    // and rgb_feat columns 0..31 in fp32 in slab 2 (columns [64,96), RF_SLAB); [0,64) is dead (pooling #1's per-point
+    // operand goes there).  In xch: the gate and rgb_feat columns 32..34.
+    tc::named_sync(BAR_LAYER, NCOMP);
+    // rgb_feat: rf[4q + i] = column 8q + 4wg + i (columns 35.. are the constant and padding, which pool to 0)
+    float rf[20];
 #pragma unroll
-    for (int s = 0; s < 3; ++s) ring.release(s);
-    ring.advance(3);
-    if (DEBUG && kp.dbg != nullptr && row_ok && wg == 0) {
-      float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
-      o[0] = mrow; o[1] = zrow; o[2] = hit; o[3] = visib; o[4] = dbg_px; o[5] = dbg_py;
-      o[6] = dbg_dir[0]; o[7] = dbg_dir[1]; o[8] = dbg_dir[2]; o[9] = rgbin[0]; o[10] = rgbin[1]; o[11] = rgbin[2];
+    for (int k = 0; k < 4; ++k) {
+      const float4 t = *reinterpret_cast<const float4*>(b.act + RF_SLAB + rf_slab_index(row, 8 * k + 4 * wg));
+      rf[4 * k] = t.x; rf[4 * k + 1] = t.y; rf[4 * k + 2] = t.z; rf[4 * k + 3] = t.w;
     }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) rf[16 + i] = wg == 0 && i < 3 ? xch[(XCH_RF + i) * 128 + row] : 0.f;
+    const float gate = xch[XCH_GATE * 128 + row];
 
     PM_TICK(6)
     // ---------------- view pooling #1 (ibrnet.py:336-339) -> the view-pooled part of base_fc.0, once per point ----------------
@@ -962,13 +1079,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       for (int j = 0; j < 16; ++j) x[j] = elu(x[j]);
       st_own<4>(b, c0, 64 + c0, x);                                                // lo half 1 lands on accumulator columns already consumed
     }
-    {
-      // the row scalars of the chain's fragment rows, into the heads' exchange slots (dead since the heads' outputs were
-      // read): w1, mrow, dd[0] from warp group 0, dd[1..3] from warp group 1
-      const float rs[6] = {w1, mrow, dd[0], dd[1], dd[2], dd[3]};
-#pragma unroll
-      for (int k = 0; k < 3; ++k) xch[(XCH_ROW + 3 * wg + k) * 128 + row] = wg ? rs[3 + k] : rs[k];
-    }
+    if (wg == 0) xch[XCH_W1 * 128 + row] = w1;                                     // w1 of the chain's fragment rows
     PM_TICK(8)
     // ---------------- base_fc.2, vis_fc, vis_fc2, rgb_fc.0: each warp group for its own 64 rows (run_chain) ----------------
     tc::fence_proxy_async_smem();
@@ -1090,7 +1201,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       const float logit = v >= rfn ? -3.0e38f : (mrow == 0.f ? -1e9f : l3);
       const float mx = gmax(logit);
       const float e = v >= rfn ? 0.f : expf(logit - mx);
-      float acc[4] = {e, e * rgbin[0], e * rgbin[1], e * rgbin[2]};
+      const float* __restrict__ rgbin_x = xch + (XCH_FRONT + 8) * 128 + row;       // this row's rgbin, as the front read it
+      float acc[4] = {e, e * rgbin_x[0], e * rgbin_x[128], e * rgbin_x[256]};
       if constexpr (P2) bsum_vec<G, 4>(acc); else gsum4_np2<G>(stg, lane, lane0, idle, acc);
       if (v == 0 && pt_ok) {
         float4* __restrict__ dst = reinterpret_cast<float4*>(pp.point_rec + size_t(n) * REC);

@@ -44,7 +44,7 @@ p.use_vis, p.var_bias, p.point_rec = 0, 0.05, rec.data_ptr()
 _lib.check(_lib.lib().nr_point_kernel_timing(C.byref(p), timing.data_ptr(), None), "timing")
 torch.cuda.synchronize()
 t = timing.cpu().reshape(64, 2, 32)
-nm = ["geom+proj", "gather", "RF->A", "dd heads", "hit/vis+pe0", "pe1+nf+raydir", "pool1+base0 per point", "base0 epilogue",
+nm = ["geom+proj", "gather", "RF->A", "dd heads", "hit/vis+pe0", "pe1+nf+base0A+raydir+base0B+handoff", "pool1+base0 per point", "base0 epilogue",
       "base1 (chain entry)", "vis0", "vis2+vis1", "v20+v21", "rgb0+exit", "pool2+geo0 per point", "geo2 (wg0) / blend (wg1) + rec"]
 for wg in (0, 1):
     d = (t[4:40, wg, 1:16] - t[4:40, wg, 0:15]).double().mean(0)
