@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 8
+#define NR_ABI_VERSION 9
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -155,6 +155,23 @@ typedef struct NrPassParams {
  * predict_proj_ray_prob + get_img_feats + network_rendering (+ ray_mask, render_depth), and optionally the
  * following sample_fine_depth.  Two kernels: point kernel (per point x view) and ray kernel (per ray). */
 int nr_render_pass_fwd(const NrPassParams* p, void* stream);
+
+/* Direct rendering of the same pass (reference renderer.py:85-125, 181-185 and sph_solver.py, cfg use_dr_prediction),
+ * forward only.  Enqueue it after nr_render_pass_fwd of the same NrPassParams: it reads the pass' inputs and, with
+ * use_nr_color, the NR colours of its point record.  Per point: the per-view alpha logits of the active pass' dist decoder
+ * (ground state where the view misses the point) pooled by visibility, and the colour of a degree-3 spherical-harmonics fit
+ * to the views' colours weighted by hit probability (regs on the normal matrix's diagonal; sph_fitter.regs of the
+ * reference) or, with use_nr_color (use_nr_color_for_dr), the NR colour; per ray: sigmoid, alpha_values2hit_prob and the
+ * colour sum.  Two kernels, no host synchronisation. */
+typedef struct NrDrParams {
+  float regs[16];            /* SphericalHarmonicsSolver(3).regs: 0, 0.001 x3, 0.005 x5, 0.05 x7 by default */
+  float alpha_ground_state;  /* cfg alpha_value_ground_state */
+  int32_t use_nr_color;      /* cfg use_nr_color_for_dr */
+  float* point_colors;       /* workspace [rn,dn,3] */
+  float* pixel_colors_dr;    /* [rn,3] */
+  float* hit_prob_dr;        /* [rn,dn] */
+} NrDrParams;
+int nr_direct_render(const NrPassParams* p, const NrDrParams* d, void* stream);
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);

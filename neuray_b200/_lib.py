@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -43,6 +43,11 @@ class NrPassParams(C.Structure):
     ]
 
 
+class NrDrParams(C.Structure):
+    _fields_ = [("regs", C.c_float * 16), ("alpha_ground_state", C.c_float), ("use_nr_color", C.c_int32),
+                ("point_colors", C.c_void_p), ("pixel_colors_dr", C.c_void_p), ("hit_prob_dr", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -70,6 +75,7 @@ SIGNATURES = {
     "nr_camera_blocks": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "nr_pack_feature_maps": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "nr_render_pass_fwd": (C.c_int, [C.POINTER(NrPassParams), _vp]),
+    "nr_direct_render": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrDrParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_debug": (C.c_int, [C.POINTER(NrPassParams), _vp, _vp]),

@@ -223,6 +223,20 @@ class RenderPassFn(torch.autograd.Function):
         return (None, None, drf if ray_feats.requires_grad else None, dimf if img_feats.requires_grad else None, *gp)
 
 
+class DirectRenderFn(torch.autograd.Function):
+    """The direct-rendering outputs of a pass (nr_direct_render) under autograd: values only.  Their gradients are not
+    implemented, so a loss on them fails loudly instead of training a model that silently ignores it."""
+
+    @staticmethod
+    def forward(ctx, dr, ray_feats, img_feats, *params):
+        return dr["pixel_colors_dr"], dr["hit_prob_dr"]
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise _lib.NeurayB200Error("the direct-rendering outputs pixel_colors_dr / hit_prob_dr have no native backward: "
+                                   "use_dr_loss / use_dr_fine_loss cannot be trained through neuray_b200")
+
+
 class SelfHitProbFn(torch.autograd.Function):
     """predict_self_hit_prob (reference renderer.py:137-155) through nr_self_hit_prob, forward and backward."""
 

@@ -241,111 +241,133 @@ NR_HD PointGeo point_geometry(const NrPassParams& pp, long long n) {
   return g;
 }
 
+// ---- one (point, view) row up to the dist decoder's probabilities (renderer.py:67-83 with project_points_dict) ------
+// Shared by the training forward (row_forward_a) and direct rendering (nr_dr_math.cuh).  `hit` and `visb` are compute_prob's
+// values BEFORE the projection mask; `dir` is project_points_directions' unit vector (ref camera -> point, negated).  With
+// `tape` non-null the heads' hidden activations go to its R_H1 / R_H2 slots of row r.
+struct RowFront {
+  float mask, dir[3];
+  float rf[32], imf[32], rgb[3], tw[4];
+  int tcode;
+  float mean[2], var[2], aw, visd, c0[2], c1[2], lo, hi, hit, visb;
+};
+NR_HD void row_front(const NrPassParams& pp, const float* __restrict__ W, int n_heads, const PointGeo& g, int v, RowFront& o,
+                     const Tape* tape, long long r) {
+  const int h = pp.h, w = pp.w, fh = pp.fh, fw = pp.fw;
+  const bool feat_align = (fh == h && fw == w);
+  const float* vp = pp.view_params + v * 20;
+  const float xh = fmaf(vp[2], g.Z, fmaf(vp[1], g.Y, vp[0] * g.X)) + vp[3];
+  const float yh = fmaf(vp[6], g.Z, fmaf(vp[5], g.Y, vp[4] * g.X)) + vp[7];
+  float zh = fmaf(vp[10], g.Z, fmaf(vp[9], g.Y, vp[8] * g.X)) + vp[11];
+  const bool degenerate = fabsf(zh) < 1e-4f;
+  if (degenerate) zh = 1e-3f;
+  const float ux = xh / zh, uy = yh / zh;
+  const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
+  const bool valid = !degenerate && !outside;
+  o.mask = valid ? 1.f : 0.f;
+  const float dx = g.X - vp[12], dy = g.Y - vp[13], dz = g.Z - vp[14];
+  const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
+  o.dir[0] = dx * inv; o.dir[1] = dy * inv; o.dir[2] = dz * inv;
+  for (int k = 0; k < 3; ++k) o.rgb[k] = 0.f;
+  for (int k = 0; k < 4; ++k) o.tw[k] = 0.f;
+  for (int k = 0; k < 32; ++k) { o.rf[k] = 0.f; o.imf[k] = 0.f; }
+  o.tcode = -1;
+  if (valid) {
+    const float gx = ux / float(w - 1) * 2.f - 1.f, gy = uy / float(h - 1) * 2.f - 1.f;
+    float fx = feat_align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
+    float fy = feat_align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
+    fx = fminf(fmaxf(fx, 0.f), float(fw - 1)); fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
+    {
+      const float x0f = floorf(fx), y0f = floorf(fy);
+      const int x0 = int(x0f), y0 = int(y0f);
+      const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
+      o.tcode = (((v * fh + y0) * fw + x0) << 6) | (x0 + 1 <= fw - 1 ? 1 : 0) | (y0 + 1 <= fh - 1 ? 2 : 0);
+      o.tw[0] = ww * wn; o.tw[1] = we * wn; o.tw[2] = ww * ws; o.tw[3] = we * ws;
+      const float* base = pp.feat + (o.tcode & ~63);
+      const int dxo = (o.tcode & 1) << 6, dyo = (o.tcode & 2) ? fw * 64 : 0;
+      for (int k = 0; k < 32; ++k) {
+        o.rf[k] = base[k] * o.tw[0] + base[dxo + k] * o.tw[1] + base[dyo + k] * o.tw[2] + base[dyo + dxo + k] * o.tw[3];
+        o.imf[k] = base[32 + k] * o.tw[0] + base[dxo + 32 + k] * o.tw[1] + base[dyo + 32 + k] * o.tw[2] + base[dyo + dxo + 32 + k] * o.tw[3];
+      }
+    }
+    {
+      float ix = (gx + 1.f) / 2.f * float(w - 1), iy = (gy + 1.f) / 2.f * float(h - 1);
+      ix = fminf(fmaxf(ix, 0.f), float(w - 1)); iy = fminf(fmaxf(iy, 0.f), float(h - 1));
+      const float x0f = floorf(ix), y0f = floorf(iy);
+      const int x0 = int(x0f), y0 = int(y0f);
+      const int x1 = x0 + 1 < w ? x0 + 1 : w - 1, y1 = y0 + 1 < h ? y0 + 1 : h - 1;
+      const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
+      const float* b = pp.rgb + (size_t)v * h * w * 4;
+      const float* t00 = b + ((size_t)y0 * w + x0) * 4; const float* t01 = b + ((size_t)y0 * w + x1) * 4;
+      const float* t10 = b + ((size_t)y1 * w + x0) * 4; const float* t11 = b + ((size_t)y1 * w + x1) * 4;
+      for (int k = 0; k < 3; ++k) o.rgb[k] = t00[k] * (ww * wn) + t01[k] * (we * wn) + t10[k] * (ww * ws) + t11[k] * (we * ws);
+    }
+  }
+
+  // dist decoder heads (dist_decoder.py:64-107)
+  float ho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
+  for (int hd = 0; hd < n_heads; ++hd) {
+    const float* Wh = W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
+    float h1[32], h2[32];
+    lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, o.rf, h1);
+    for (int k = 0; k < 32; ++k) h1[k] = elu_f(h1[k]);
+    lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1, h2);
+    for (int k = 0; k < 32; ++k) h2[k] = elu_f(h2[k]);
+    if (tape) {
+      stv<32>(*tape, R_H1 + 32 * hd, r, h1);
+      stv<32>(*tape, R_H2 + 32 * hd, r, h2);
+    }
+    for (int oo = 0; oo < 2; ++oo) {
+      float a = Wh[lay::DD_L2_B + oo];
+      for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + oo * 32 + k], h2[k], a);
+      ho[hd][oo] = a;
+    }
+  }
+  for (int i = 0; i < 2; ++i) { o.mean[i] = softplus_f(ho[0][i]); o.var[i] = softplus_f(ho[1][i]) + pp.var_bias; }
+  o.aw = sigm(ho[2][0]);
+  o.visd = pp.use_vis ? sigm(ho[3][0]) : 1.f;
+  // compute_prob (dist_decoder.py:6-51, 109-140)
+  const float zc = fmaxf(zh, 1e-5f);
+  const float tz = (-1.f / zc - vp[15]) / (vp[16] - vp[15]);
+  o.lo = tz - g.ihp; o.hi = tz + g.ihc;
+  o.hit = 0.f; o.visb = 0.f;
+  for (int i = 0; i < 2; ++i) {
+    o.c0[i] = sigm(2.f * (o.lo - o.mean[i]) * o.var[i]);      // 0.5 + 0.5 tanh(x)
+    o.c1[i] = sigm(2.f * (o.hi - o.mean[i]) * o.var[i]);
+    const float mix = i == 0 ? o.aw : 1.f - o.aw;
+    o.visb += (1.f - o.c0[i] * o.visd) * mix;
+    o.hit += (o.c1[i] - o.c0[i]) * o.visd * mix;
+  }
+}
+
 // ---- forward, phase a, one (point, view) row: gather, dist decoder, probabilities, prob_embed, neuray_fc, ray_dir_fc ----
 NR_HD void row_forward_a(const Ctx& c, long long r) {
   const NrPassParams& pp = c.p;
   const float* __restrict__ W = c.W;
-  const int h = pp.h, w = pp.w, fh = pp.fh, fw = pp.fw;
   const long long N = (long long)pp.rn * pp.dn;
   const int v = int(r / N);
   const long long n = r - (long long)v * N;
-  const bool feat_align = (fh == h && fw == w);
   const PointGeo g = point_geometry(pp, n);
   {
-    const float* vp = pp.view_params + v * 20;
-    const float xh = fmaf(vp[2], g.Z, fmaf(vp[1], g.Y, vp[0] * g.X)) + vp[3];
-    const float yh = fmaf(vp[6], g.Z, fmaf(vp[5], g.Y, vp[4] * g.X)) + vp[7];
-    float zh = fmaf(vp[10], g.Z, fmaf(vp[9], g.Y, vp[8] * g.X)) + vp[11];
-    const bool degenerate = fabsf(zh) < 1e-4f;
-    if (degenerate) zh = 1e-3f;
-    const float ux = xh / zh, uy = yh / zh;
-    const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
-    const bool valid = !degenerate && !outside;
-    const float mask = valid ? 1.f : 0.f;
-    const float dx = g.X - vp[12], dy = g.Y - vp[13], dz = g.Z - vp[14];
-    const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
-    const float ex = dx * inv, ey = dy * inv, ez = dz * inv;
-    float dd[4] = {ex - g.qx, ey - g.qy, ez - g.qz, ex * g.qx + ey * g.qy + ez * g.qz};
-    float rf[32], imf[32], rgb[3] = {0.f, 0.f, 0.f}, tw[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int k = 0; k < 32; ++k) { rf[k] = 0.f; imf[k] = 0.f; }
-    int tcode = -1;
-    if (valid) {
-      const float gx = ux / float(w - 1) * 2.f - 1.f, gy = uy / float(h - 1) * 2.f - 1.f;
-      float fx = feat_align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-      float fy = feat_align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-      fx = fminf(fmaxf(fx, 0.f), float(fw - 1)); fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
-      {
-        const float x0f = floorf(fx), y0f = floorf(fy);
-        const int x0 = int(x0f), y0 = int(y0f);
-        const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
-        tcode = (((v * fh + y0) * fw + x0) << 6) | (x0 + 1 <= fw - 1 ? 1 : 0) | (y0 + 1 <= fh - 1 ? 2 : 0);
-        tw[0] = ww * wn; tw[1] = we * wn; tw[2] = ww * ws; tw[3] = we * ws;
-        const float* base = pp.feat + (tcode & ~63);
-        const int dxo = (tcode & 1) << 6, dyo = (tcode & 2) ? fw * 64 : 0;
-        for (int k = 0; k < 32; ++k) {
-          rf[k] = base[k] * tw[0] + base[dxo + k] * tw[1] + base[dyo + k] * tw[2] + base[dyo + dxo + k] * tw[3];
-          imf[k] = base[32 + k] * tw[0] + base[dxo + 32 + k] * tw[1] + base[dyo + 32 + k] * tw[2] + base[dyo + dxo + 32 + k] * tw[3];
-        }
-      }
-      {
-        float ix = (gx + 1.f) / 2.f * float(w - 1), iy = (gy + 1.f) / 2.f * float(h - 1);
-        ix = fminf(fmaxf(ix, 0.f), float(w - 1)); iy = fminf(fmaxf(iy, 0.f), float(h - 1));
-        const float x0f = floorf(ix), y0f = floorf(iy);
-        const int x0 = int(x0f), y0 = int(y0f);
-        const int x1 = x0 + 1 < w ? x0 + 1 : w - 1, y1 = y0 + 1 < h ? y0 + 1 : h - 1;
-        const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
-        const float* b = pp.rgb + (size_t)v * h * w * 4;
-        const float* t00 = b + ((size_t)y0 * w + x0) * 4; const float* t01 = b + ((size_t)y0 * w + x1) * 4;
-        const float* t10 = b + ((size_t)y1 * w + x0) * 4; const float* t11 = b + ((size_t)y1 * w + x1) * 4;
-        for (int k = 0; k < 3; ++k) rgb[k] = t00[k] * (ww * wn) + t01[k] * (we * wn) + t10[k] * (ww * ws) + t11[k] * (we * ws);
-      }
-    }
+    RowFront f;
+    row_front(pp, W, c.n_heads, g, v, f, &c.tr, r);
+    const float mask = f.mask;
+    const float* rf = f.rf;
+    const float* imf = f.imf;
+    const float* rgb = f.rgb;
+    float dd[4] = {f.dir[0] - g.qx, f.dir[1] - g.qy, f.dir[2] - g.qz, f.dir[0] * g.qx + f.dir[1] * g.qy + f.dir[2] * g.qz};
     stv<32>(c.tr, R_RF, r, rf);
     stv<4>(c.tr, R_DD, r, dd);
     stv<4>(c.tr, R_DDC, r, dd);
     stv<3>(c.tr, R_RGB, r, rgb);
-    stv<4>(c.tr, R_TW, r, tw);
-    { float tc; memcpy(&tc, &tcode, 4); c.tr.at(R_TCODE, r) = tc; }
+    stv<4>(c.tr, R_TW, r, f.tw);
+    { float tc; memcpy(&tc, &f.tcode, 4); c.tr.at(R_TCODE, r) = tc; }
     c.tr.at(R_MASK, r) = mask;
-
-    // dist decoder heads (dist_decoder.py:64-107)
-    float ho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
-    for (int hd = 0; hd < c.n_heads; ++hd) {
-      const float* Wh = W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
-      float h1[32], h2[32];
-      lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, rf, h1);
-      for (int k = 0; k < 32; ++k) h1[k] = elu_f(h1[k]);
-      lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1, h2);
-      for (int k = 0; k < 32; ++k) h2[k] = elu_f(h2[k]);
-      stv<32>(c.tr, R_H1 + 32 * hd, r, h1);
-      stv<32>(c.tr, R_H2 + 32 * hd, r, h2);
-      for (int o = 0; o < 2; ++o) {
-        float a = Wh[lay::DD_L2_B + o];
-        for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + o * 32 + k], h2[k], a);
-        ho[hd][o] = a;
-      }
-    }
-    float mean[2], var[2];
-    for (int i = 0; i < 2; ++i) { mean[i] = softplus_f(ho[0][i]); var[i] = softplus_f(ho[1][i]) + pp.var_bias; }
-    const float aw = sigm(ho[2][0]);
-    const float visd = pp.use_vis ? sigm(ho[3][0]) : 1.f;
-    // compute_prob (dist_decoder.py:6-51, 109-140)
-    const float zc = fmaxf(zh, 1e-5f);
-    const float tz = (-1.f / zc - vp[15]) / (vp[16] - vp[15]);
-    const float lo = tz - g.ihp, hi = tz + g.ihc;
-    float c0[2], c1[2], hit = 0.f, visb = 0.f;
-    for (int i = 0; i < 2; ++i) {
-      c0[i] = sigm(2.f * (lo - mean[i]) * var[i]);      // 0.5 + 0.5 tanh(x)
-      c1[i] = sigm(2.f * (hi - mean[i]) * var[i]);
-      const float mix = i == 0 ? aw : 1.f - aw;
-      visb += (1.f - c0[i] * visd) * mix;
-      hit += (c1[i] - c0[i]) * visd * mix;
-    }
-    visb *= mask; hit *= mask;
-    stv<2>(c.tr, R_MEAN, r, mean); stv<2>(c.tr, R_VAR, r, var);
-    c.tr.at(R_AW, r) = aw; c.tr.at(R_VISD, r) = visd;
-    stv<2>(c.tr, R_C0, r, c0); stv<2>(c.tr, R_C1, r, c1);
-    c.tr.at(R_TLO, r) = lo; c.tr.at(R_THI, r) = hi;
+    const float visb = f.visb * mask, hit = f.hit * mask;
+    stv<2>(c.tr, R_MEAN, r, f.mean); stv<2>(c.tr, R_VAR, r, f.var);
+    c.tr.at(R_AW, r) = f.aw; c.tr.at(R_VISD, r) = f.visd;
+    stv<2>(c.tr, R_C0, r, f.c0); stv<2>(c.tr, R_C1, r, f.c1);
+    c.tr.at(R_TLO, r) = f.lo; c.tr.at(R_THI, r) = f.hi;
     const float hitn = (hit - 0.5f) * 2.f, visn = (visb - 0.5f) * 2.f;
     c.tr.at(R_HITN, r) = hitn; c.tr.at(R_VISN, r) = visn;
 

@@ -192,10 +192,45 @@ def pass_index_map(owner, is_fine, dev):
     return maps[key]
 
 
-def _check_supported(owner):
-    cfg = owner.cfg
-    if cfg.get("use_dr_prediction", False):
-        raise NotImplementedError("use_dr_prediction (direct rendering / SH fit) is outside the native hot path (SURVEY.md 8f)")
+# SphericalHarmonicsSolver(3).regs (reference sph_solver.py:6-12): the diagonal added to the SH fit's normal matrix
+_SH_REGS = (0.0,) + (0.001,) * 3 + (0.005,) * 5 + (0.05,) * 7
+
+
+def _sh_regs(owner):
+    """The owner's sph_fitter.regs (read once per buffer version), or the solver's constructor defaults."""
+    fitter = getattr(owner, "sph_fitter", None)
+    if fitter is None:
+        return _SH_REGS
+    regs = fitter.regs
+    stamp = (regs.data_ptr(), regs._version)
+    hit = owner.__dict__.get("_nr_sh_regs")
+    if hit is None or hit[0] != stamp:
+        if regs.numel() != len(_SH_REGS):
+            raise _lib.NeurayB200Error(f"sph_fitter.regs has {regs.numel()} entries: direct rendering fits degree 3 (16)")
+        hit = (stamp, tuple(float(x) for x in regs.detach().float().cpu()))
+        owner.__dict__["_nr_sh_regs"] = hit
+    return hit[1]
+
+
+def _direct_render(owner, out, rn, dn, dev):
+    """use_dr_prediction (reference renderer.py:85-125, 181-185): nr_direct_render enqueued right behind the pass whose raw
+    outputs `out` holds, while that pass' point record is still in the shared workspace.  Returns pixel_colors_dr [1,rn,3]
+    and hit_prob_dr [1,rn,dn]."""
+    res = {"pixel_colors_dr": torch.empty(1, rn, 3, dtype=torch.float32, device=dev),
+           "hit_prob_dr": torch.empty(1, rn, dn, dtype=torch.float32, device=dev)}
+    if out["_bwd"] is None:          # rn == 0: nothing was launched
+        return res
+    p, _keep, _, stream = out["_bwd"]
+    d = _lib.NrDrParams()
+    d.regs[:] = _sh_regs(owner)
+    d.alpha_ground_state = float(owner.cfg["alpha_value_ground_state"])
+    d.use_nr_color = 1 if owner.cfg["use_nr_color_for_dr"] else 0
+    d.point_colors = _lib.ptr(_workspace("dr_point_colors", rn * dn * 3, dev))
+    d.pixel_colors_dr, d.hit_prob_dr = _lib.ptr(res["pixel_colors_dr"]), _lib.ptr(res["hit_prob_dr"])
+    with _lib.on_device(res["hit_prob_dr"]):
+        _lib.check(_lib.lib().nr_direct_render(C.byref(p), C.byref(d), stream), "nr_direct_render")
+    _lib.count_launches(2)
+    return res
 
 
 def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit):
@@ -265,11 +300,11 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
 def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None, want_hit=True):
     """One fused pass.  que_depth [1,rn,dn].  `fine`: None or dict(dn=, use_all=, u=, u_stride=) to also emit the
     next pass' depths.  Returns dict with pixel_colors [1,rn,3], hit_prob [1,rn,dn], render_depth [1,rn],
-    ray_mask [1,rn] (bool) and optionally fine_depth [1,rn,M].
+    ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M] and, with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
+    hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels)."""
-    _check_supported(owner)
     coords = que_imgs_info["coords"]
     if coords.shape[0] != 1:
         raise _lib.NeurayB200Error("one query view per call (qn == 1), like every call site of the reference")
@@ -281,7 +316,13 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     rf, imf = ref_imgs_info["ray_feats"], ref_imgs_info["img_feats"]
     named = [(f"{dec_name}.{k}", v) for k, v in dec.named_parameters()] + [(f"{agg_name}.{k}", v) for k, v in agg.named_parameters()]
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for _, v in named))
-    launch = lambda: _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit)
+    dr = {} if owner.cfg["use_dr_prediction"] else None
+
+    def launch():
+        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit)
+        if dr is not None:
+            dr.update(_direct_render(owner, out, rn, dn, coords.device))
+        return out
     if not needs_grad:
         out = launch()
         out.pop("_bwd", None)
@@ -292,6 +333,11 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
         out = {"pixel_colors": res[0], "hit_prob": res[1], "render_depth": res[2], "ray_mask_u8": res[3]}
         if fine:
             out["fine_depth"] = res[4]
+        if dr is not None:
+            from .backward import DirectRenderFn
+            dr = dict(zip(("pixel_colors_dr", "hit_prob_dr"), DirectRenderFn.apply(dr, rf, imf, *[v for _, v in named])))
+    if dr is not None:
+        out.update(dr)
     out["ray_mask"] = out.pop("ray_mask_u8").bool()
     return out
 
@@ -299,6 +345,8 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
 def _finish_outputs(owner, res, que_depth, que_imgs_info):
     cfg = owner.cfg
     outputs = {"pixel_colors_nr": res["pixel_colors"], "hit_prob_nr": res["hit_prob"]}
+    if cfg["use_dr_prediction"]:
+        outputs["pixel_colors_dr"], outputs["hit_prob_dr"] = res["pixel_colors_dr"], res["hit_prob_dr"]
     if "imgs" in que_imgs_info:
         outputs["pixel_colors_gt"] = interpolate_feats(que_imgs_info["imgs"], que_imgs_info["coords"], align_corners=True)
     if cfg["use_ray_mask"]:
