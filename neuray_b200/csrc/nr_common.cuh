@@ -6,6 +6,8 @@
 
 #include "../../include/neuray_b200.h"
 
+#define NR_HD __host__ __device__ __forceinline__
+
 namespace nr {
 
 void set_error(const char* fmt, ...);
@@ -183,6 +185,105 @@ __device__ __forceinline__ float softplusf_(float x) { return x > 20.f ? x : fma
 __device__ __forceinline__ float logistic_cdf(float x) {
   // 0.5 + 0.5*tanh(x) = 1/(1+exp(-2x))
   return 1.f / (1.f + __expf(-2.f * x));
+}
+
+// read-only input: the non-coherent load path on the device
+NR_HD float ld_ro(const float* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
+// ---- geometry of one query point (render_ops.py coords2rays / depth2points, dist_decoder.py get_near_far_points) ---------
+// Point n = ray * dn + s: its world position on ray `ray` at que_depth[n], the unit query direction (camera -> point,
+// negated) and the half widths of its bin towards the previous / next sample in normalised inverse depth.  cam: the query
+// camera block of NrPassParams::que_cam, wherever the caller keeps it.
+struct PointGeo { float X, Y, Z, qx, qy, qz, ihp, ihc; };
+template <typename I>
+NR_HD PointGeo point_geometry(const float* cam, const float* coords, const float* que_depth, int dn, I n) {
+  PointGeo g;
+  const I ray = n / dn;
+  const int s = int(n - ray * dn);
+  const float cx = ld_ro(coords + 2 * ray), cy = ld_ro(coords + 2 * ray + 1);
+  float cm[3], d[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) cm[i] = fmaf(cam[12 + 3 * i + 1], cy, cam[12 + 3 * i] * cx) + cam[12 + 3 * i + 2];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const float wld = fmaf(cam[3 * i + 2], cm[2], fmaf(cam[3 * i + 1], cm[1], cam[3 * i] * cm[0])) + cam[9 + i];
+    d[i] = wld - cam[9 + i];   // the reference adds the centre and subtracts it again (render_ops.py:22-23)
+  }
+  const float z = ld_ro(que_depth + n);
+  g.X = fmaf(d[0], z, cam[9]); g.Y = fmaf(d[1], z, cam[10]); g.Z = fmaf(d[2], z, cam[11]);
+  const float nrm = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+  g.qx = -d[0] / nrm; g.qy = -d[1] / nrm; g.qz = -d[2] / nrm;
+  const float a = -1.f / cam[21], bb = -1.f / cam[22];
+  const float tcur = (-1.f / z - a) / (bb - a);
+  float dc = 1e6f;
+  if (s + 1 < dn) dc = (-1.f / ld_ro(que_depth + n + 1) - a) / (bb - a) - tcur;
+  float dp = dc;
+  if (s > 0) dp = tcur - (-1.f / ld_ro(que_depth + n - 1) - a) / (bb - a);
+  g.ihc = dc * 0.5f; g.ihp = dp * 0.5f;
+  return g;
+}
+
+// ---- projection of a point into a view of an h x w image (render_ops.py project_points_dict) ----------------------------
+// vp: the view's 20-float row of NrPassParams::view_params.  zh is the projected depth after the fix-up of a point on the
+// camera plane; valid_z is false for such a point, valid also for one outside the image.  dir: the unit vector view centre
+// -> point, negated (project_points_directions).
+struct Proj {
+  float ux, uy, zh, dir[3];
+  bool valid, valid_z;
+};
+NR_HD Proj project(const float* vp, float X, float Y, float Z, int h, int w) {
+  Proj p;
+  const float xh = fmaf(vp[2], Z, fmaf(vp[1], Y, vp[0] * X)) + vp[3];
+  const float yh = fmaf(vp[6], Z, fmaf(vp[5], Y, vp[4] * X)) + vp[7];
+  float zh = fmaf(vp[10], Z, fmaf(vp[9], Y, vp[8] * X)) + vp[11];
+  const bool degenerate = fabsf(zh) < 1e-4f;
+  if (degenerate) zh = 1e-3f;
+  p.ux = xh / zh; p.uy = yh / zh; p.zh = zh;
+  const bool outside = (p.ux < -0.5f) || (p.ux >= float(w) - 0.5f) || (p.uy < -0.5f) || (p.uy >= float(h) - 0.5f);
+  p.valid_z = !degenerate;
+  p.valid = !degenerate && !outside;
+  const float dx = X - vp[12], dy = Y - vp[13], dz = Z - vp[14];
+  const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
+  p.dir[0] = dx * inv; p.dir[1] = dy * inv; p.dir[2] = dz * inv;
+  return p;
+}
+
+// ---- bilinear taps of interpolate_feats (ops.py:14-34) with padding_mode='border' ---------------------------------------
+// Coordinates (x, y) in pixels of an h x w image, sampled from an fh x fw map; align_corners when the map is full
+// resolution (render_ops.py:54-70).  Texel columns x0 <= x1 and rows y0 <= y1, weights of (y0,x0), (y0,x1), (y1,x0), (y1,x1).
+struct Taps {
+  int x0, x1, y0, y1;
+  float w[4];
+};
+NR_HD Taps border_taps(float x, float y, int h, int w, int fh, int fw, bool align) {
+  const float gx = x / float(w - 1) * 2.f - 1.f, gy = y / float(h - 1) * 2.f - 1.f;
+  float fx = align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
+  float fy = align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
+  fx = fminf(fmaxf(fx, 0.f), float(fw - 1));
+  fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
+  const float x0f = floorf(fx), y0f = floorf(fy);
+  Taps t;
+  t.x0 = int(x0f); t.y0 = int(y0f);
+  t.x1 = t.x0 + 1 < fw ? t.x0 + 1 : fw - 1; t.y1 = t.y0 + 1 < fh ? t.y0 + 1 : fh - 1;
+  const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
+  t.w[0] = ww * wn; t.w[1] = we * wn; t.w[2] = ww * ws; t.w[3] = we * ws;
+  return t;
+}
+// the taps applied to one fw-wide plane
+NR_HD float bilinear(const float* plane, int fw, const Taps& t) {
+  return plane[t.y0 * fw + t.x0] * t.w[0] + plane[t.y0 * fw + t.x1] * t.w[1] + plane[t.y1 * fw + t.x0] * t.w[2] +
+         plane[t.y1 * fw + t.x1] * t.w[3];
+}
+// the taps in view v of the channel-last [rfn, fh, fw, 64] feature maps: element offset of the (y0,x0) texel (a multiple
+// of 64) with "x1 > x0" / "y1 > y0" in its two low bits
+NR_HD int tap_code(const Taps& t, int v, int fh, int fw) {
+  return (((v * fh + t.y0) * fw + t.x0) << 6) | (t.x1 > t.x0 ? 1 : 0) | (t.y1 > t.y0 ? 2 : 0);
 }
 
 }  // namespace nr

@@ -107,7 +107,7 @@ NR_HD void sh_fit_color(const float* rows, int stride, int rfn, float hit_sum, c
 NR_HD void dr_point(const NrPassParams& pp, const NrDrParams& d, const float* __restrict__ W, long long n, float* rows, int stride,
                     float* alpha_out, float* color_out) {
   const int n_heads = pp.use_vis ? 4 : 3;
-  const tr::PointGeo g = tr::point_geometry(pp, n);
+  const PointGeo g = point_geometry(pp.que_cam, pp.coords, pp.que_depth, pp.dn, n);
   float hit_sum = 0.f, vis_sum = 0.f, va_sum = 0.f, mask_sum = 0.f;
   for (int v = 0; v < pp.rfn; ++v) {
     tr::RowFront f;

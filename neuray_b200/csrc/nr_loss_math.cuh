@@ -12,33 +12,10 @@ namespace nr {
 namespace ls {
 
 using tr::atomic_add;
-using tr::elu_f;
-using tr::elu_g;
-using tr::lin;
-using tr::lin_t;
+using tr::head_bwd;
+using tr::head_fwd;
 using tr::softplus_f;
-
-// bilinear taps of interpolate_feats (ops.py:14-34) with padding_mode='border': coordinates (x, y) in pixels of an h x w
-// image, sampled from an fh x fw map; align_corners when the map is full resolution (render_ops.py:54-70)
-struct Taps {
-  int off[4];
-  float w[4];
-};
-NR_HD Taps border_taps(float x, float y, int h, int w, int fh, int fw, bool align) {
-  const float gx = x / float(w - 1) * 2.f - 1.f, gy = y / float(h - 1) * 2.f - 1.f;
-  float fx = align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-  float fy = align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-  fx = fminf(fmaxf(fx, 0.f), float(fw - 1));
-  fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
-  const float x0f = floorf(fx), y0f = floorf(fy);
-  const int x0 = int(x0f), y0 = int(y0f);
-  const int x1 = x0 + 1 < fw ? x0 + 1 : fw - 1, y1 = y0 + 1 < fh ? y0 + 1 : fh - 1;
-  const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
-  Taps t;
-  t.w[0] = ww * wn; t.w[1] = we * wn; t.w[2] = ww * ws; t.w[3] = we * ws;
-  t.off[0] = y0 * fw + x0; t.off[1] = y0 * fw + x1; t.off[2] = y1 * fw + x0; t.off[3] = y1 * fw + x1;
-  return t;
-}
+using tr::softplus_g;
 
 // ---- predict_mean_for_depth_loss ----------------------------------------------------------------------------------------
 typedef NrDepthMeanParams DepthMeanP;   // include/neuray_b200.h
@@ -52,55 +29,30 @@ NR_HD void depth_mean_point(const DepthMeanP& p, long long i) {
   const float* map = p.map + (size_t)view * 32 * fh * fw;
   const Taps t = border_taps(p.coords[2 * i], p.coords[2 * i + 1], p.h, p.w, fh, fw, fh == p.h && fw == p.w);
   float rf[32];
-  for (int k = 0; k < 32; ++k) {
-    const float* m = map + (size_t)k * fh * fw;
-    rf[k] = m[t.off[0]] * t.w[0] + m[t.off[1]] * t.w[1] + m[t.off[2]] * t.w[2] + m[t.off[3]] * t.w[3];
-  }
+  for (int k = 0; k < 32; ++k) rf[k] = bilinear(map + (size_t)k * fh * fw, fw, t);
   float drf[32];
   for (int k = 0; k < 32; ++k) drf[k] = 0.f;
   bool any_grad = false;
   for (int d = 0; d < 2; ++d) {
     if (p.w_point[d] == nullptr) continue;
     const float* Wh = p.w_point[d] + lay::DD_HEAD;   // head 0 = mean decoder
-    float h1[32], h2[32];
-    lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, rf, h1);
-    for (int k = 0; k < 32; ++k) h1[k] = elu_f(h1[k]);
-    lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1, h2);
-    for (int k = 0; k < 32; ++k) h2[k] = elu_f(h2[k]);
-    float mean[2];
+    float h1[32], h2[32], ho[2], mean[2];
+    head_fwd(Wh, rf, h1, h2, ho, nullptr, 0, 0);
     for (int o = 0; o < 2; ++o) {
-      float a = Wh[lay::DD_L2_B + o];
-      for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + o * 32 + k], h2[k], a);
-      mean[o] = softplus_f(a);
+      mean[o] = softplus_f(ho[o]);
       if (p.mean[d] != nullptr) p.mean[d][2 * i + o] = mean[o];
     }
     if (p.d_mean[d] == nullptr) continue;
     any_grad = true;
-    float* dWh = p.d_w_point[d] + lay::DD_HEAD;
-    float dho[2], dz1[32], dz0[32], tt[32];
-    for (int o = 0; o < 2; ++o) dho[o] = p.d_mean[d][2 * i + o] * (1.f - expf(-mean[o]));     // softplus' = sigmoid(x) = 1 - exp(-softplus(x))
-    for (int o = 0; o < 2; ++o) {
-      atomic_add(dWh + lay::DD_L2_B + o, dho[o]);
-      for (int k = 0; k < 32; ++k) atomic_add(dWh + lay::DD_L2_W + o * 32 + k, dho[o] * h2[k]);
-    }
-    for (int k = 0; k < 32; ++k) dz1[k] = (Wh[lay::DD_L2_W + k] * dho[0] + Wh[lay::DD_L2_W + 32 + k] * dho[1]) * elu_g(h2[k]);
-    lin_t<32, 32>(Wh + lay::DD_L1_W, dz1, dz0);
-    for (int k = 0; k < 32; ++k) dz0[k] *= elu_g(h1[k]);
-    for (int j = 0; j < 32; ++j) {
-      atomic_add(dWh + lay::DD_L1_B + j, dz1[j]);
-      atomic_add(dWh + lay::DD_L0_B + j, dz0[j]);
-      for (int k = 0; k < 32; ++k) {                                  // WT[in][out]
-        atomic_add(dWh + lay::DD_L1_W + k * 32 + j, h1[k] * dz1[j]);
-        atomic_add(dWh + lay::DD_L0_W + k * 32 + j, rf[k] * dz0[j]);
-      }
-    }
-    lin_t<32, 32>(Wh + lay::DD_L0_W, dz0, tt);
-    for (int k = 0; k < 32; ++k) drf[k] += tt[k];
+    float dho[2];
+    for (int o = 0; o < 2; ++o) dho[o] = p.d_mean[d][2 * i + o] * softplus_g(mean[o]);
+    head_bwd(Wh, rf, h1, h2, dho, drf, p.d_w_point[d] + lay::DD_HEAD, nullptr, 0, 0);
   }
   if (any_grad && p.d_map != nullptr) {
+    const int off[4] = {t.y0 * fw + t.x0, t.y0 * fw + t.x1, t.y1 * fw + t.x0, t.y1 * fw + t.x1};
     float* dm = p.d_map + (size_t)view * 32 * fh * fw;
     for (int k = 0; k < 32; ++k)
-      for (int q = 0; q < 4; ++q) atomic_add(dm + (size_t)k * fh * fw + t.off[q], drf[k] * t.w[q]);
+      for (int q = 0; q < 4; ++q) atomic_add(dm + (size_t)k * fh * fw + off[q], drf[k] * t.w[q]);
   }
 }
 
@@ -121,8 +73,7 @@ NR_HD float depth_process(float depth, float near, float far) {
   return fminf(fmaxf(depth, 0.f), 1.f);
 }
 NR_HD float depth_at(const float* map, const float* coords, long long i, int h, int w) {
-  const Taps t = border_taps(coords[2 * i], coords[2 * i + 1], h, w, h, w, true);
-  return map[t.off[0]] * t.w[0] + map[t.off[1]] * t.w[1] + map[t.off[2]] * t.w[2] + map[t.off[3]] * t.w[3];
+  return bilinear(map, w, border_taps(coords[2 * i], coords[2 * i + 1], h, w, h, w, true));
 }
 // loss term and its derivative with respect to the prediction; mask (1 unless the 'gso' consistency mask applies)
 NR_HD void depth_loss_term(const DepthLossP& p, long long i, const float* depth_pr, float& term, float& dterm, float& mask) {

@@ -13,10 +13,6 @@
 
 #include "nr_common.cuh"
 
-#ifndef NR_HD
-#define NR_HD __host__ __device__ __forceinline__
-#endif
-
 namespace nr {
 namespace mvs {
 

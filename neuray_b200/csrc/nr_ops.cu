@@ -129,57 +129,59 @@ __global__ void project_kernel(const float* __restrict__ pts, long long pn, cons
   const long long total = pn * rfn;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long v = i / pn, n = i - v * pn;
-    const float* __restrict__ vp = vps + v * 20;
-    const float X = pts[3 * n], Y = pts[3 * n + 1], Z = pts[3 * n + 2];
-    const float xh = fmaf(vp[2], Z, fmaf(vp[1], Y, vp[0] * X)) + vp[3];
-    const float yh = fmaf(vp[6], Z, fmaf(vp[5], Y, vp[4] * X)) + vp[7];
-    float zh = fmaf(vp[10], Z, fmaf(vp[9], Y, vp[8] * X)) + vp[11];
-    const bool degenerate = fabsf(zh) < 1e-4f;
-    if (degenerate) zh = 1e-3f;
-    const float ux = xh / zh, uy = yh / zh;
-    const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
-    if (pix) { pix[2 * i] = ux; pix[2 * i + 1] = uy; }
-    if (depth) depth[i] = zh;
-    if (mask) mask[i] = (!degenerate && !outside) ? 1.f : 0.f;
-    if (valid_z) valid_z[i] = degenerate ? 0.f : 1.f;
-    if (dir) {
-      const float dx = X - vp[12], dy = Y - vp[13], dz = Z - vp[14];
-      const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
-      dir[3 * i] = dx * inv; dir[3 * i + 1] = dy * inv; dir[3 * i + 2] = dz * inv;
-    }
+    const Proj pj = project(vps + v * 20, pts[3 * n], pts[3 * n + 1], pts[3 * n + 2], h, w);
+    if (pix) { pix[2 * i] = pj.ux; pix[2 * i + 1] = pj.uy; }
+    if (depth) depth[i] = pj.zh;
+    if (mask) mask[i] = pj.valid ? 1.f : 0.f;
+    if (valid_z) valid_z[i] = pj.valid_z ? 1.f : 0.f;
+    if (dir) { dir[3 * i] = pj.dir[0]; dir[3 * i + 1] = pj.dir[1]; dir[3 * i + 2] = pj.dir[2]; }
   }
 }
 
 // ---- bilinear sampling on an NCHW map (F.grid_sample semantics through ops.py:14-34) --------------------------
+// Taps at pixel (x, y) of an h x w image on an fh x fw map: the texel columns xa, xb and rows ya, yb, clamped into the map,
+// and the weights of (ya,xa), (ya,xb), (yb,xa), (yb,xb) times `scale`.  A texel outside the map (zeros padding) or a
+// non-finite coordinate contributes nothing: its weight is 0.
+struct InterpTaps {
+  int xa, xb, ya, yb;
+  float w00, w01, w10, w11;
+};
+__device__ __forceinline__ InterpTaps interp_taps(float x, float y, float h, float w, int fh, int fw, int border, int align,
+                                                  float scale) {
+  const float gx = x / (w - 1.f) * 2.f - 1.f, gy = y / (h - 1.f) * 2.f - 1.f;
+  float ix = align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
+  float iy = align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
+  if (border) {
+    ix = fminf(fmaxf(ix, 0.f), float(fw - 1));
+    iy = fminf(fmaxf(iy, 0.f), float(fh - 1));
+  }
+  const float x0f = floorf(ix), y0f = floorf(iy);
+  const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
+  const bool finite = fabsf(x0f) < 1e9f && fabsf(y0f) < 1e9f;
+  const int x0 = finite ? int(x0f) : -10, y0 = finite ? int(y0f) : -10;
+  const bool vx0 = x0 >= 0 && x0 < fw, vx1 = x0 + 1 >= 0 && x0 + 1 < fw;
+  const bool vy0 = y0 >= 0 && y0 < fh, vy1 = y0 + 1 >= 0 && y0 + 1 < fh;
+  InterpTaps t;
+  t.w00 = (vx0 && vy0) ? ww * wn * scale : 0.f; t.w01 = (vx1 && vy0) ? we * wn * scale : 0.f;
+  t.w10 = (vx0 && vy1) ? ww * ws * scale : 0.f; t.w11 = (vx1 && vy1) ? we * ws * scale : 0.f;
+  t.xa = min(max(x0, 0), fw - 1); t.xb = min(max(x0 + 1, 0), fw - 1);
+  t.ya = min(max(y0, 0), fh - 1); t.yb = min(max(y0 + 1, 0), fh - 1);
+  return t;
+}
+
 __global__ void interp_kernel(const float* __restrict__ feats, const float* __restrict__ pts, const float* __restrict__ mask,
                               int b, int c, int fh, int fw, long long n, float h, float w, int border, int align,
                               float* __restrict__ out) {
   const long long total = (long long)b * n;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long bi = i / n;
-    const float gx = pts[2 * i] / (w - 1.f) * 2.f - 1.f, gy = pts[2 * i + 1] / (h - 1.f) * 2.f - 1.f;
-    float ix = align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-    float iy = align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-    if (border) {
-      ix = fminf(fmaxf(ix, 0.f), float(fw - 1));
-      iy = fminf(fmaxf(iy, 0.f), float(fh - 1));
-    }
-    const float x0f = floorf(ix), y0f = floorf(iy);
-    const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
-    // out-of-range coordinates (zeros padding, or non-finite) contribute nothing
-    const bool finite = fabsf(x0f) < 1e9f && fabsf(y0f) < 1e9f;
-    const int x0 = finite ? int(x0f) : -10, y0 = finite ? int(y0f) : -10;
-    const bool vx0 = x0 >= 0 && x0 < fw, vx1 = x0 + 1 >= 0 && x0 + 1 < fw;
-    const bool vy0 = y0 >= 0 && y0 < fh, vy1 = y0 + 1 >= 0 && y0 + 1 < fh;
-    const float w00 = (vx0 && vy0) ? ww * wn : 0.f, w01 = (vx1 && vy0) ? we * wn : 0.f;
-    const float w10 = (vx0 && vy1) ? ww * ws : 0.f, w11 = (vx1 && vy1) ? we * ws : 0.f;
-    const int xa = min(max(x0, 0), fw - 1), xb = min(max(x0 + 1, 0), fw - 1);
-    const int ya = min(max(y0, 0), fh - 1), yb = min(max(y0 + 1, 0), fh - 1);
+    const InterpTaps t = interp_taps(pts[2 * i], pts[2 * i + 1], h, w, fh, fw, border, align, 1.f);
     const float m = mask ? mask[i] : 1.f;
     const float* __restrict__ base = feats + bi * c * fh * fw;
     for (int ch = 0; ch < c; ++ch) {
       const float* __restrict__ pl = base + (long long)ch * fh * fw;
-      const float val = pl[ya * fw + xa] * w00 + pl[ya * fw + xb] * w01 + pl[yb * fw + xa] * w10 + pl[yb * fw + xb] * w11;
+      const float val = pl[t.ya * fw + t.xa] * t.w00 + pl[t.ya * fw + t.xb] * t.w01 + pl[t.yb * fw + t.xa] * t.w10 +
+                        pl[t.yb * fw + t.xb] * t.w11;
       out[i * c + ch] = val * m;
     }
   }
@@ -193,32 +195,15 @@ __global__ void interp_bwd_kernel(const float* __restrict__ d_out, const float* 
   const long long total = (long long)b * n;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long bi = i / n;
-    const float gx = pts[2 * i] / (w - 1.f) * 2.f - 1.f, gy = pts[2 * i + 1] / (h - 1.f) * 2.f - 1.f;
-    float ix = align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-    float iy = align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-    if (border) {
-      ix = fminf(fmaxf(ix, 0.f), float(fw - 1));
-      iy = fminf(fmaxf(iy, 0.f), float(fh - 1));
-    }
-    const float x0f = floorf(ix), y0f = floorf(iy);
-    const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
-    const bool finite = fabsf(x0f) < 1e9f && fabsf(y0f) < 1e9f;
-    const int x0 = finite ? int(x0f) : -10, y0 = finite ? int(y0f) : -10;
-    const bool vx0 = x0 >= 0 && x0 < fw, vx1 = x0 + 1 >= 0 && x0 + 1 < fw;
-    const bool vy0 = y0 >= 0 && y0 < fh, vy1 = y0 + 1 >= 0 && y0 + 1 < fh;
-    const float m = mask ? mask[i] : 1.f;
-    const float w00 = (vx0 && vy0) ? ww * wn * m : 0.f, w01 = (vx1 && vy0) ? we * wn * m : 0.f;
-    const float w10 = (vx0 && vy1) ? ww * ws * m : 0.f, w11 = (vx1 && vy1) ? we * ws * m : 0.f;
-    const int xa = min(max(x0, 0), fw - 1), xb = min(max(x0 + 1, 0), fw - 1);
-    const int ya = min(max(y0, 0), fh - 1), yb = min(max(y0 + 1, 0), fh - 1);
+    const InterpTaps t = interp_taps(pts[2 * i], pts[2 * i + 1], h, w, fh, fw, border, align, mask ? mask[i] : 1.f);
     float* __restrict__ base = d_feats + bi * c * fh * fw;
     for (int ch = 0; ch < c; ++ch) {
       float* __restrict__ pl = base + (long long)ch * fh * fw;
       const float g = d_out[i * c + ch];
-      if (w00 != 0.f) atomicAdd(pl + ya * fw + xa, g * w00);
-      if (w01 != 0.f) atomicAdd(pl + ya * fw + xb, g * w01);
-      if (w10 != 0.f) atomicAdd(pl + yb * fw + xa, g * w10);
-      if (w11 != 0.f) atomicAdd(pl + yb * fw + xb, g * w11);
+      if (t.w00 != 0.f) atomicAdd(pl + t.ya * fw + t.xa, g * t.w00);
+      if (t.w01 != 0.f) atomicAdd(pl + t.ya * fw + t.xb, g * t.w01);
+      if (t.w10 != 0.f) atomicAdd(pl + t.yb * fw + t.xa, g * t.w10);
+      if (t.w11 != 0.f) atomicAdd(pl + t.yb * fw + t.xb, g * t.w11);
     }
   }
 }
@@ -437,11 +422,6 @@ int nr_sample_fine_depth(const float* depth, const float* hit_prob, const float*
 namespace nr {
 namespace ops {
 
-__device__ __forceinline__ float bil1(const float* __restrict__ pl, int w, int xa, int xb, int ya, int yb, float w00, float w01, float w10,
-                                      float w11) {
-  return pl[ya * w + xa] * w00 + pl[ya * w + xb] * w01 + pl[yb * w + xa] * w10 + pl[yb * w + xb] * w11;
-}
-
 __global__ void diff_feats_kernel(const float* __restrict__ imgs, const float* __restrict__ depth_in, const float* __restrict__ poses,
                                   const float* __restrict__ Ks, const float* __restrict__ vps, int rfn, int h, int w,
                                   float* __restrict__ out) {
@@ -480,32 +460,22 @@ __global__ void diff_feats_kernel(const float* __restrict__ imgs, const float* _
     float n = 0.f, s[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
     for (int j = 0; j < rfn; ++j) {
       const float* __restrict__ vp = vps + j * 20;
-      const float xh = fmaf(vp[2], X[2], fmaf(vp[1], X[1], vp[0] * X[0])) + vp[3];
-      const float yh = fmaf(vp[6], X[2], fmaf(vp[5], X[1], vp[4] * X[0])) + vp[7];
-      float zh = fmaf(vp[10], X[2], fmaf(vp[9], X[1], vp[8] * X[0])) + vp[11];
-      const bool degenerate = fabsf(zh) < 1e-4f;
-      if (degenerate) zh = 1e-3f;
-      const float ux = xh / zh, uy = yh / zh;
-      const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
-      if (degenerate || outside) continue;
+      const Proj pj = project(vp, X[0], X[1], X[2], h, w);
+      if (!pj.valid) continue;
       // bilinear, border clamp, align_corners (interpolate_feats(..., padding_mode='border', align_corners=True))
-      float ix = (ux / float(w - 1) * 2.f - 1.f + 1.f) / 2.f * float(w - 1), iy = (uy / float(h - 1) * 2.f - 1.f + 1.f) / 2.f * float(h - 1);
-      ix = fminf(fmaxf(ix, 0.f), float(w - 1)); iy = fminf(fmaxf(iy, 0.f), float(h - 1));
-      const float x0f = floorf(ix), y0f = floorf(iy);
-      const int xa = int(x0f), ya = int(y0f), xb = min(xa + 1, w - 1), yb = min(ya + 1, h - 1);
-      const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
-      const float w00 = ww * wn, w01 = we * wn, w10 = ww * ws, w11 = we * ws;
+      const Taps t = border_taps(pj.ux, pj.uy, h, w, h, w, true);
       const float* __restrict__ img = imgs + (long long)j * 3 * hw;
-      const float dr = fabsf(bil1(img, w, xa, xb, ya, yb, w00, w01, w10, w11) - r0);
-      const float dg = fabsf(bil1(img + hw, w, xa, xb, ya, yb, w00, w01, w10, w11) - g0);
-      const float db = fabsf(bil1(img + 2 * hw, w, xa, xb, ya, yb, w00, w01, w10, w11) - b0);
+      const float dr = fabsf(bilinear(img, w, t) - r0);
+      const float dg = fabsf(bilinear(img + hw, w, t) - g0);
+      const float db = fabsf(bilinear(img + 2 * hw, w, t) - b0);
       // depth map of view j: the reference samples the METRIC depth of view j (depth = -1/depth_in with view j's range)
       const float* __restrict__ dj = depth_in + (long long)j * hw;
       const float nj = vp[15], fj = vp[16];
       auto metric = [&](float t) { return -1.f / (t * (fj - nj) + nj); };
-      const float dint = metric(dj[ya * w + xa]) * w00 + metric(dj[ya * w + xb]) * w01 + metric(dj[yb * w + xa]) * w10 + metric(dj[yb * w + xb]) * w11;
+      const float dint = metric(dj[t.y0 * w + t.x0]) * t.w[0] + metric(dj[t.y0 * w + t.x1]) * t.w[1] + metric(dj[t.y1 * w + t.x0]) * t.w[2] +
+                         metric(dj[t.y1 * w + t.x1]) * t.w[3];
       // normalised by the range of the view projected INTO (init_net.py:49-50: near/far broadcast over the first axis = j)
-      const float dd = fminf(fabsf(-1.f / fmaxf(dint, 1e-5f) + 1.f / fmaxf(zh, 1e-5f)) / (fj - nj), 1.5f);
+      const float dd = fminf(fabsf(-1.f / fmaxf(dint, 1e-5f) + 1.f / fmaxf(pj.zh, 1e-5f)) / (fj - nj), 1.5f);
       n += 1.f;
       s[0] += dr; s[1] += dg; s[2] += db; s[3] += dd;
       s2[0] = fmaf(dr, dr, s2[0]); s2[1] = fmaf(dg, dg, s2[1]); s2[2] = fmaf(db, db, s2[2]); s2[3] = fmaf(dd, dd, s2[3]);

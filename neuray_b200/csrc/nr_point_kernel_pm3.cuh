@@ -650,78 +650,31 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 
     PM_TICK(0)
     // ---------------- ray geometry of this row's point (every lane of the group, in both warp groups, computes the same values) ----------------
-    float X = 0.f, Y = 0.f, Z = 0.f, qx = 0.f, qy = 0.f, qz = 0.f, ihp = 0.f, ihc = 0.f;
-    if (pt_ok) {
-      const float* cam = smem + OFF_CAM;
-      const int ray = n / dn, s = n - ray * dn;
-      const float cx = __ldg(pp.coords + 2 * ray), cy = __ldg(pp.coords + 2 * ray + 1);
-      float cm[3], d[3];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) cm[i] = fmaf(cam[12 + 3 * i + 1], cy, cam[12 + 3 * i] * cx) + cam[12 + 3 * i + 2];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const float wld = fmaf(cam[3 * i + 2], cm[2], fmaf(cam[3 * i + 1], cm[1], cam[3 * i] * cm[0])) + cam[9 + i];
-        d[i] = wld - cam[9 + i];   // the reference adds the centre and subtracts it again (render_ops.py:22-23)
-      }
-      const float z = __ldg(pp.que_depth + n);
-      X = fmaf(d[0], z, cam[9]); Y = fmaf(d[1], z, cam[10]); Z = fmaf(d[2], z, cam[11]);
-      const float nrm = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-      qx = -d[0] / nrm; qy = -d[1] / nrm; qz = -d[2] / nrm;
-      const float a = -1.f / cam[21], bb = -1.f / cam[22];
-      const float tcur = (-1.f / z - a) / (bb - a);
-      float dc = 1e6f;
-      if (s + 1 < dn) dc = (-1.f / __ldg(pp.que_depth + n + 1) - a) / (bb - a) - tcur;
-      float dp = dc;
-      if (s > 0) dp = tcur - (-1.f / __ldg(pp.que_depth + n - 1) - a) / (bb - a);
-      ihc = dc * 0.5f; ihp = dp * 0.5f;
-    }
+    PointGeo geo = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (pt_ok) geo = point_geometry(smem + OFF_CAM, pp.coords, pp.que_depth, dn, n);
 
-    // ---------------- projection into this row's view + rgb taps ----------------
-    float mrow = 0.f, zrow = 1.f, dd[4] = {0.f, 0.f, 0.f, 0.f}, fxr = 0.f, fyr = 0.f, rgbin[3] = {0.f, 0.f, 0.f};
+    // ---------------- projection into this row's view + feature and rgb taps ----------------
+    float mrow = 0.f, zrow = 1.f, dd[4] = {0.f, 0.f, 0.f, 0.f}, rgbin[3] = {0.f, 0.f, 0.f};
     float dbg_px = 0.f, dbg_py = 0.f, dbg_dir[3] = {0.f, 0.f, 0.f};
     int tcode = -1;
     float tw[4] = {0.f, 0.f, 0.f, 0.f};
     if (row_ok) {
-      const float* vp = smem + OFF_CAM + 32 + v * 20;
-      const float xh = fmaf(vp[2], Z, fmaf(vp[1], Y, vp[0] * X)) + vp[3];
-      const float yh = fmaf(vp[6], Z, fmaf(vp[5], Y, vp[4] * X)) + vp[7];
-      float zh = fmaf(vp[10], Z, fmaf(vp[9], Y, vp[8] * X)) + vp[11];
-      const bool degenerate = fabsf(zh) < 1e-4f;
-      if (degenerate) zh = 1e-3f;
-      const float ux = xh / zh, uy = yh / zh;
-      const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
-      const bool valid = !degenerate && !outside;
-      mrow = valid ? 1.f : 0.f;
-      zrow = zh;
-      const float dx = X - vp[12], dy = Y - vp[13], dz = Z - vp[14];
-      const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
-      const float ex = dx * inv, ey = dy * inv, ez = dz * inv;
-      dd[0] = ex - qx; dd[1] = ey - qy; dd[2] = ez - qz; dd[3] = ex * qx + ey * qy + ez * qz;
-      if (DEBUG) { dbg_px = ux; dbg_py = uy; dbg_dir[0] = ex; dbg_dir[1] = ey; dbg_dir[2] = ez; }
-      const float gx = ux / float(w - 1) * 2.f - 1.f, gy = uy / float(h - 1) * 2.f - 1.f;
-      fxr = feat_align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-      fyr = feat_align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-      fxr = fminf(fmaxf(fxr, 0.f), float(fw - 1)); fyr = fminf(fmaxf(fyr, 0.f), float(fh - 1));
-      if (valid) {
-        // feature-map taps of this row, worked out once here instead of by each of the gathering lanes: element offset
-        // of the (y0,x0) texel (a multiple of 64) with "x1 > x0" / "y1 > y0" in its two low bits, and the four weights
-        const float x0f = floorf(fxr), y0f = floorf(fyr);
-        const int x0 = int(x0f), y0 = int(y0f);
-        const float we = fxr - x0f, ww = (x0f + 1.f) - fxr, ws = fyr - y0f, wn = (y0f + 1.f) - fyr;
-        tcode = (((v * fh + y0) * fw + x0) << 6) | (x0 + 1 <= fw - 1 ? 1 : 0) | (y0 + 1 <= fh - 1 ? 2 : 0);
-        tw[0] = ww * wn; tw[1] = we * wn; tw[2] = ww * ws; tw[3] = we * ws;
-      }
-      if (valid) {
-        float ix = (gx + 1.f) / 2.f * float(w - 1), iy = (gy + 1.f) / 2.f * float(h - 1);
-        ix = fminf(fmaxf(ix, 0.f), float(w - 1)); iy = fminf(fmaxf(iy, 0.f), float(h - 1));
-        const float x0f = floorf(ix), y0f = floorf(iy);
-        const int x0 = int(x0f), y0 = int(y0f);
-        const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-        const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
+      const Proj pj = project(smem + OFF_CAM + 32 + v * 20, geo.X, geo.Y, geo.Z, h, w);
+      mrow = pj.valid ? 1.f : 0.f;
+      zrow = pj.zh;
+      const float ex = pj.dir[0], ey = pj.dir[1], ez = pj.dir[2];
+      dd[0] = ex - geo.qx; dd[1] = ey - geo.qy; dd[2] = ez - geo.qz; dd[3] = ex * geo.qx + ey * geo.qy + ez * geo.qz;
+      if (DEBUG) { dbg_px = pj.ux; dbg_py = pj.uy; dbg_dir[0] = ex; dbg_dir[1] = ey; dbg_dir[2] = ez; }
+      if (pj.valid) {
+        // feature-map taps of this row, worked out once here instead of by each of the gathering lanes
+        const Taps ft = border_taps(pj.ux, pj.uy, h, w, fh, fw, feat_align);
+        tcode = tap_code(ft, v, fh, fw);
+        tw[0] = ft.w[0]; tw[1] = ft.w[1]; tw[2] = ft.w[2]; tw[3] = ft.w[3];
+        const Taps rt = border_taps(pj.ux, pj.uy, h, w, h, w, true);
         const float* __restrict__ base = pp.rgb + size_t(v) * h * w * 4;
-        const float4 t00 = ldg4(base + (size_t(y0) * w + x0) * 4), t01 = ldg4(base + (size_t(y0) * w + x1) * 4);
-        const float4 t10 = ldg4(base + (size_t(y1) * w + x0) * 4), t11 = ldg4(base + (size_t(y1) * w + x1) * 4);
-        const float w00 = ww * wn, w01 = we * wn, w10 = ww * ws, w11 = we * ws;
+        const float4 t00 = ldg4(base + (size_t(rt.y0) * w + rt.x0) * 4), t01 = ldg4(base + (size_t(rt.y0) * w + rt.x1) * 4);
+        const float4 t10 = ldg4(base + (size_t(rt.y1) * w + rt.x0) * 4), t11 = ldg4(base + (size_t(rt.y1) * w + rt.x1) * 4);
+        const float w00 = rt.w[0], w01 = rt.w[1], w10 = rt.w[2], w11 = rt.w[3];
         rgbin[0] = t00.x * w00 + t01.x * w01 + t10.x * w10 + t11.x * w11;
         rgbin[1] = t00.y * w00 + t01.y * w01 + t10.y * w10 + t11.y * w11;
         rgbin[2] = t00.z * w00 + t01.z * w01 + t10.z * w10 + t11.z * w11;
@@ -792,7 +745,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     {
       // the row scalars of the front's fragment rows, read after the heads: zrow, ihp, ihc, mrow, dd[0..1] from warp
       // group 0, dd[2..3], rgbin[0..2] from warp group 1
-      const float rs[11] = {zrow, ihp, ihc, mrow, dd[0], dd[1], dd[2], dd[3], rgbin[0], rgbin[1], rgbin[2]};
+      const float rs[11] = {zrow, geo.ihp, geo.ihc, mrow, dd[0], dd[1], dd[2], dd[3], rgbin[0], rgbin[1], rgbin[2]};
 #pragma unroll
       for (int k = 0; k < 5; ++k) xch[(XCH_FRONT + 6 * wg + k) * 128 + row] = wg ? rs[6 + k] : rs[k];
       if (wg == 0) xch[(XCH_FRONT + 5) * 128 + row] = rs[5];

@@ -24,8 +24,6 @@
 namespace nr {
 namespace tr {
 
-#define NR_HD __host__ __device__ __forceinline__
-
 // ---- tape slots -------------------------------------------------------------------------------------------------
 enum RowSlot {
   R_RF = 0,        // 32 gathered ray_feats (x mask)
@@ -151,6 +149,7 @@ NR_HD float elu_f(float x) { return x > 0.f ? x : expf(x) - 1.f; }
 NR_HD float elu_g(float a) { return a > 0.f ? 1.f : a + 1.f; }           // derivative from the activation's output
 NR_HD float sigm(float x) { return 1.f / (1.f + expf(-x)); }
 NR_HD float softplus_f(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+NR_HD float softplus_g(float a) { return 1.f - expf(-a); }               // derivative from the activation's output
 
 // z[OUT] = b + W^T x with W stored [IN][LD].  Weight rows are read with 128-bit loads when the shapes allow (all
 // weight blocks start on 16-byte boundaries, nr_common.cuh lay::): every thread reads the same addresses, so the load
@@ -212,33 +211,100 @@ NR_HD void atomic_add4(float* p, float a, float b, float c, float d) {
 #endif
 }
 
-// ---- geometry of one point and its projection into one view (same expressions as the forward point kernel) --------
-struct PointGeo { float X, Y, Z, qx, qy, qz, ihp, ihc; };
-NR_HD PointGeo point_geometry(const NrPassParams& pp, long long n) {
-  PointGeo g;
-  const float* cam = pp.que_cam;
-  const int dn = pp.dn;
-  const long long ray = n / dn;
-  const int s = int(n - ray * dn);
-  const float cx = pp.coords[2 * ray], cy = pp.coords[2 * ray + 1];
-  float cm[3], d[3];
-  for (int i = 0; i < 3; ++i) cm[i] = fmaf(cam[12 + 3 * i + 1], cy, cam[12 + 3 * i] * cx) + cam[12 + 3 * i + 2];
-  for (int i = 0; i < 3; ++i) {
-    const float wld = fmaf(cam[3 * i + 2], cm[2], fmaf(cam[3 * i + 1], cm[1], cam[3 * i] * cm[0])) + cam[9 + i];
-    d[i] = wld - cam[9 + i];
+// ---- one dist-decoder head (dist_decoder.py:64-97): Linear(32,32) ELU Linear(32,32) ELU Linear(32,2) ------------------
+// Wh: head hd's block of w_point (lay::DD_*); h1, h2: the two ELU outputs.  With `tape` non-null the forward writes h1 / h2
+// to its R_H1 / R_H2 slots of row r, and the backward dz1 / dz0 to its G_DD1 / G_DD0 slots; with `dWh` non-null the
+// backward adds the weight gradients to dWh (laid out like Wh) by atomics.  Both happen where the values are made: a
+// store after the call would keep 32 more values live and spill in the 255-register training kernels.
+NR_HD void head_fwd(const float* __restrict__ Wh, const float* rf, float* h1, float* h2, float* out, const Tape* tape, long long r,
+                    int hd) {
+  lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, rf, h1);
+  for (int k = 0; k < 32; ++k) h1[k] = elu_f(h1[k]);
+  lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1, h2);
+  for (int k = 0; k < 32; ++k) h2[k] = elu_f(h2[k]);
+  if (tape) {
+    stv<32>(*tape, R_H1 + 32 * hd, r, h1);
+    stv<32>(*tape, R_H2 + 32 * hd, r, h2);
   }
-  const float z = pp.que_depth[n];
-  g.X = fmaf(d[0], z, cam[9]); g.Y = fmaf(d[1], z, cam[10]); g.Z = fmaf(d[2], z, cam[11]);
-  const float nrm = sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-  g.qx = -d[0] / nrm; g.qy = -d[1] / nrm; g.qz = -d[2] / nrm;
-  const float a = -1.f / cam[21], bb = -1.f / cam[22];
-  const float tcur = (-1.f / z - a) / (bb - a);
-  float dc = 1e6f;
-  if (s + 1 < dn) dc = (-1.f / pp.que_depth[n + 1] - a) / (bb - a) - tcur;
-  float dp = dc;
-  if (s > 0) dp = tcur - (-1.f / pp.que_depth[n - 1] - a) / (bb - a);
-  g.ihc = dc * 0.5f; g.ihp = dp * 0.5f;
-  return g;
+  for (int o = 0; o < 2; ++o) {
+    float a = Wh[lay::DD_L2_B + o];
+    for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + o * 32 + k], h2[k], a);
+    out[o] = a;
+  }
+}
+// Backward from the output gradients dho: W0 dz0 is added to drf (rf, the head's input, is read only with dWh).
+NR_HD void head_bwd(const float* __restrict__ Wh, const float* rf, const float* h1, const float* h2, const float* dho, float* drf,
+                    float* dWh, const Tape* tape, long long r, int hd) {
+  if (dWh)
+    for (int o = 0; o < 2; ++o) {
+      atomic_add(dWh + lay::DD_L2_B + o, dho[o]);
+      for (int k = 0; k < 32; ++k) atomic_add(dWh + lay::DD_L2_W + o * 32 + k, dho[o] * h2[k]);
+    }
+  float dz1[32], dz0[32], t[32];
+  for (int k = 0; k < 32; ++k) dz1[k] = (Wh[lay::DD_L2_W + k] * dho[0] + Wh[lay::DD_L2_W + 32 + k] * dho[1]) * elu_g(h2[k]);
+  if (tape) stv<32>(*tape, G_DD1 + 32 * hd, r, dz1);
+  lin_t<32, 32>(Wh + lay::DD_L1_W, dz1, dz0);
+  for (int k = 0; k < 32; ++k) dz0[k] *= elu_g(h1[k]);
+  if (tape) stv<32>(*tape, G_DD0 + 32 * hd, r, dz0);
+  if (dWh)
+    for (int j = 0; j < 32; ++j) {
+      atomic_add(dWh + lay::DD_L1_B + j, dz1[j]);
+      atomic_add(dWh + lay::DD_L0_B + j, dz0[j]);
+      for (int i = 0; i < 32; ++i) {                                // WT[in][out]
+        atomic_add(dWh + lay::DD_L1_W + i * 32 + j, h1[i] * dz1[j]);
+        atomic_add(dWh + lay::DD_L0_W + i * 32 + j, rf[i] * dz0[j]);
+      }
+    }
+  lin_t<32, 32>(Wh + lay::DD_L0_W, dz0, t);
+  for (int k = 0; k < 32; ++k) drf[k] += t[k];
+}
+
+// ---- compute_prob (dist_decoder.py:6-51, 109-140) ----------------------------------------------------------------------
+// The two-component mixture from the heads' outputs ho (mean, var, aw, vis; ho[3] is read only with use_vis).
+struct Mix { float mean[2], var[2], aw, visd; };
+NR_HD Mix mix_fwd(const float (&ho)[4][2], float var_bias, bool use_vis) {
+  Mix m;
+  for (int i = 0; i < 2; ++i) { m.mean[i] = softplus_f(ho[0][i]); m.var[i] = softplus_f(ho[1][i]) + var_bias; }
+  m.aw = sigm(ho[2][0]);
+  m.visd = use_vis ? sigm(ho[3][0]) : 1.f;
+  return m;
+}
+// Hit and visibility of the bin (lo, hi) in normalised inverse depth, before any projection mask; c0 / c1: each
+// component's CDF at lo / hi, before the vis factor.
+NR_HD void bin_fwd(const Mix& m, float lo, float hi, float* c0, float* c1, float& hit, float& visb) {
+  hit = 0.f; visb = 0.f;
+  for (int i = 0; i < 2; ++i) {
+    c0[i] = sigm(2.f * (lo - m.mean[i]) * m.var[i]);      // 0.5 + 0.5 tanh(x)
+    c1[i] = sigm(2.f * (hi - m.mean[i]) * m.var[i]);
+    const float mix = i == 0 ? m.aw : 1.f - m.aw;
+    visb += (1.f - c0[i] * m.visd) * mix;
+    hit += (c1[i] - c0[i]) * m.visd * mix;
+  }
+}
+// Gradients of the mixture's parameters (mix: of the two component weights aw, 1 - aw).
+struct MixGrad { float mean[2], var[2], mix[2], visd; };
+// bin_fwd's backward: the gradients of (hit, visb) added to g.
+NR_HD void bin_bwd(const Mix& m, float lo, float hi, const float* c0, const float* c1, float dhit, float dvisb, MixGrad& g) {
+  for (int i = 0; i < 2; ++i) {
+    const float mix = i == 0 ? m.aw : 1.f - m.aw;
+    const float dc1 = dhit * mix, dc0 = -(dhit + dvisb) * mix;          // wrt cdf * visd
+    g.mix[i] += dhit * (c1[i] - c0[i]) * m.visd + dvisb * (1.f - c0[i] * m.visd);
+    g.visd += dc1 * c1[i] + dc0 * c0[i];
+    const float dx1 = dc1 * m.visd * 2.f * c1[i] * (1.f - c1[i]), dx0 = dc0 * m.visd * 2.f * c0[i] * (1.f - c0[i]);
+    g.mean[i] -= (dx1 + dx0) * m.var[i];
+    g.var[i] += dx1 * (hi - m.mean[i]) + dx0 * (lo - m.mean[i]);
+  }
+}
+// mix_fwd's backward: the gradients of the heads' outputs (zero for ho[3] without use_vis).
+NR_HD void mix_bwd(const Mix& m, const MixGrad& g, float var_bias, bool use_vis, float (&dho)[4][2]) {
+  for (int i = 0; i < 2; ++i) {
+    dho[0][i] = g.mean[i] * softplus_g(m.mean[i]);
+    dho[1][i] = g.var[i] * softplus_g(m.var[i] - var_bias);
+  }
+  dho[2][0] = (g.mix[0] - g.mix[1]) * m.aw * (1.f - m.aw);
+  dho[2][1] = 0.f;
+  dho[3][0] = use_vis ? g.visd * m.visd * (1.f - m.visd) : 0.f;
+  dho[3][1] = 0.f;
 }
 
 // ---- one (point, view) row up to the dist decoder's probabilities (renderer.py:67-83 with project_points_dict) ------
@@ -249,40 +315,25 @@ struct RowFront {
   float mask, dir[3];
   float rf[32], imf[32], rgb[3], tw[4];
   int tcode;
-  float mean[2], var[2], aw, visd, c0[2], c1[2], lo, hi, hit, visb;
+  Mix m;
+  float c0[2], c1[2], lo, hi, hit, visb;
 };
 NR_HD void row_front(const NrPassParams& pp, const float* __restrict__ W, int n_heads, const PointGeo& g, int v, RowFront& o,
                      const Tape* tape, long long r) {
   const int h = pp.h, w = pp.w, fh = pp.fh, fw = pp.fw;
-  const bool feat_align = (fh == h && fw == w);
   const float* vp = pp.view_params + v * 20;
-  const float xh = fmaf(vp[2], g.Z, fmaf(vp[1], g.Y, vp[0] * g.X)) + vp[3];
-  const float yh = fmaf(vp[6], g.Z, fmaf(vp[5], g.Y, vp[4] * g.X)) + vp[7];
-  float zh = fmaf(vp[10], g.Z, fmaf(vp[9], g.Y, vp[8] * g.X)) + vp[11];
-  const bool degenerate = fabsf(zh) < 1e-4f;
-  if (degenerate) zh = 1e-3f;
-  const float ux = xh / zh, uy = yh / zh;
-  const bool outside = (ux < -0.5f) || (ux >= float(w) - 0.5f) || (uy < -0.5f) || (uy >= float(h) - 0.5f);
-  const bool valid = !degenerate && !outside;
-  o.mask = valid ? 1.f : 0.f;
-  const float dx = g.X - vp[12], dy = g.Y - vp[13], dz = g.Z - vp[14];
-  const float inv = -1.f / fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-5f);
-  o.dir[0] = dx * inv; o.dir[1] = dy * inv; o.dir[2] = dz * inv;
+  const Proj pj = project(vp, g.X, g.Y, g.Z, h, w);
+  o.mask = pj.valid ? 1.f : 0.f;
+  for (int k = 0; k < 3; ++k) o.dir[k] = pj.dir[k];
   for (int k = 0; k < 3; ++k) o.rgb[k] = 0.f;
   for (int k = 0; k < 4; ++k) o.tw[k] = 0.f;
   for (int k = 0; k < 32; ++k) { o.rf[k] = 0.f; o.imf[k] = 0.f; }
   o.tcode = -1;
-  if (valid) {
-    const float gx = ux / float(w - 1) * 2.f - 1.f, gy = uy / float(h - 1) * 2.f - 1.f;
-    float fx = feat_align ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-    float fy = feat_align ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-    fx = fminf(fmaxf(fx, 0.f), float(fw - 1)); fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
+  if (pj.valid) {
     {
-      const float x0f = floorf(fx), y0f = floorf(fy);
-      const int x0 = int(x0f), y0 = int(y0f);
-      const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
-      o.tcode = (((v * fh + y0) * fw + x0) << 6) | (x0 + 1 <= fw - 1 ? 1 : 0) | (y0 + 1 <= fh - 1 ? 2 : 0);
-      o.tw[0] = ww * wn; o.tw[1] = we * wn; o.tw[2] = ww * ws; o.tw[3] = we * ws;
+      const Taps t = border_taps(pj.ux, pj.uy, h, w, fh, fw, fh == h && fw == w);
+      o.tcode = tap_code(t, v, fh, fw);
+      for (int k = 0; k < 4; ++k) o.tw[k] = t.w[k];
       const float* base = pp.feat + (o.tcode & ~63);
       const int dxo = (o.tcode & 1) << 6, dyo = (o.tcode & 2) ? fw * 64 : 0;
       for (int k = 0; k < 32; ++k) {
@@ -291,53 +342,25 @@ NR_HD void row_front(const NrPassParams& pp, const float* __restrict__ W, int n_
       }
     }
     {
-      float ix = (gx + 1.f) / 2.f * float(w - 1), iy = (gy + 1.f) / 2.f * float(h - 1);
-      ix = fminf(fmaxf(ix, 0.f), float(w - 1)); iy = fminf(fmaxf(iy, 0.f), float(h - 1));
-      const float x0f = floorf(ix), y0f = floorf(iy);
-      const int x0 = int(x0f), y0 = int(y0f);
-      const int x1 = x0 + 1 < w ? x0 + 1 : w - 1, y1 = y0 + 1 < h ? y0 + 1 : h - 1;
-      const float we = ix - x0f, ww = (x0f + 1.f) - ix, ws = iy - y0f, wn = (y0f + 1.f) - iy;
+      const Taps t = border_taps(pj.ux, pj.uy, h, w, h, w, true);
       const float* b = pp.rgb + (size_t)v * h * w * 4;
-      const float* t00 = b + ((size_t)y0 * w + x0) * 4; const float* t01 = b + ((size_t)y0 * w + x1) * 4;
-      const float* t10 = b + ((size_t)y1 * w + x0) * 4; const float* t11 = b + ((size_t)y1 * w + x1) * 4;
-      for (int k = 0; k < 3; ++k) o.rgb[k] = t00[k] * (ww * wn) + t01[k] * (we * wn) + t10[k] * (ww * ws) + t11[k] * (we * ws);
+      const float* t00 = b + ((size_t)t.y0 * w + t.x0) * 4; const float* t01 = b + ((size_t)t.y0 * w + t.x1) * 4;
+      const float* t10 = b + ((size_t)t.y1 * w + t.x0) * 4; const float* t11 = b + ((size_t)t.y1 * w + t.x1) * 4;
+      for (int k = 0; k < 3; ++k) o.rgb[k] = t00[k] * t.w[0] + t01[k] * t.w[1] + t10[k] * t.w[2] + t11[k] * t.w[3];
     }
   }
 
   // dist decoder heads (dist_decoder.py:64-107)
   float ho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
   for (int hd = 0; hd < n_heads; ++hd) {
-    const float* Wh = W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
     float h1[32], h2[32];
-    lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, o.rf, h1);
-    for (int k = 0; k < 32; ++k) h1[k] = elu_f(h1[k]);
-    lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1, h2);
-    for (int k = 0; k < 32; ++k) h2[k] = elu_f(h2[k]);
-    if (tape) {
-      stv<32>(*tape, R_H1 + 32 * hd, r, h1);
-      stv<32>(*tape, R_H2 + 32 * hd, r, h2);
-    }
-    for (int oo = 0; oo < 2; ++oo) {
-      float a = Wh[lay::DD_L2_B + oo];
-      for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + oo * 32 + k], h2[k], a);
-      ho[hd][oo] = a;
-    }
+    head_fwd(W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE, o.rf, h1, h2, ho[hd], tape, r, hd);
   }
-  for (int i = 0; i < 2; ++i) { o.mean[i] = softplus_f(ho[0][i]); o.var[i] = softplus_f(ho[1][i]) + pp.var_bias; }
-  o.aw = sigm(ho[2][0]);
-  o.visd = pp.use_vis ? sigm(ho[3][0]) : 1.f;
-  // compute_prob (dist_decoder.py:6-51, 109-140)
-  const float zc = fmaxf(zh, 1e-5f);
+  o.m = mix_fwd(ho, pp.var_bias, pp.use_vis);
+  const float zc = fmaxf(pj.zh, 1e-5f);
   const float tz = (-1.f / zc - vp[15]) / (vp[16] - vp[15]);
   o.lo = tz - g.ihp; o.hi = tz + g.ihc;
-  o.hit = 0.f; o.visb = 0.f;
-  for (int i = 0; i < 2; ++i) {
-    o.c0[i] = sigm(2.f * (o.lo - o.mean[i]) * o.var[i]);      // 0.5 + 0.5 tanh(x)
-    o.c1[i] = sigm(2.f * (o.hi - o.mean[i]) * o.var[i]);
-    const float mix = i == 0 ? o.aw : 1.f - o.aw;
-    o.visb += (1.f - o.c0[i] * o.visd) * mix;
-    o.hit += (o.c1[i] - o.c0[i]) * o.visd * mix;
-  }
+  bin_fwd(o.m, o.lo, o.hi, o.c0, o.c1, o.hit, o.visb);
 }
 
 // ---- forward, phase a, one (point, view) row: gather, dist decoder, probabilities, prob_embed, neuray_fc, ray_dir_fc ----
@@ -347,7 +370,7 @@ NR_HD void row_forward_a(const Ctx& c, long long r) {
   const long long N = (long long)pp.rn * pp.dn;
   const int v = int(r / N);
   const long long n = r - (long long)v * N;
-  const PointGeo g = point_geometry(pp, n);
+  const PointGeo g = point_geometry(pp.que_cam, pp.coords, pp.que_depth, pp.dn, n);
   {
     RowFront f;
     row_front(pp, W, c.n_heads, g, v, f, &c.tr, r);
@@ -364,8 +387,8 @@ NR_HD void row_forward_a(const Ctx& c, long long r) {
     { float tc; memcpy(&tc, &f.tcode, 4); c.tr.at(R_TCODE, r) = tc; }
     c.tr.at(R_MASK, r) = mask;
     const float visb = f.visb * mask, hit = f.hit * mask;
-    stv<2>(c.tr, R_MEAN, r, f.mean); stv<2>(c.tr, R_VAR, r, f.var);
-    c.tr.at(R_AW, r) = f.aw; c.tr.at(R_VISD, r) = f.visd;
+    stv<2>(c.tr, R_MEAN, r, f.m.mean); stv<2>(c.tr, R_VAR, r, f.m.var);
+    c.tr.at(R_AW, r) = f.m.aw; c.tr.at(R_VISD, r) = f.m.visd;
     stv<2>(c.tr, R_C0, r, f.c0); stv<2>(c.tr, R_C1, r, f.c1);
     c.tr.at(R_TLO, r) = f.lo; c.tr.at(R_THI, r) = f.hi;
     const float hitn = (hit - 0.5f) * 2.f, visn = (visb - 0.5f) * 2.f;
@@ -978,41 +1001,23 @@ NR_HD void row_backward_d(const Ctx& c, long long r) {
       dhitn = de[32]; dvisn = de[33];
     }
     // compute_prob
-    float dho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
+    float dho[4][2];
     {
-      const float dhit = 2.f * dhitn * mask, dvisb = 2.f * dvisn * mask;
-      float mean[2], var[2], c0[2], c1[2];
-      ldv<2>(c.tr, R_MEAN, r, mean); ldv<2>(c.tr, R_VAR, r, var); ldv<2>(c.tr, R_C0, r, c0); ldv<2>(c.tr, R_C1, r, c1);
-      const float aw = c.tr.at(R_AW, r), visd = c.tr.at(R_VISD, r), lo = c.tr.at(R_TLO, r), hi = c.tr.at(R_THI, r);
-      float dvisd = 0.f, dmix[2];
-      for (int i = 0; i < 2; ++i) {
-        const float mix = i == 0 ? aw : 1.f - aw;
-        const float dc1 = dhit * mix, dc0 = -(dhit + dvisb) * mix;          // wrt cdf * visd
-        dmix[i] = dhit * (c1[i] - c0[i]) * visd + dvisb * (1.f - c0[i] * visd);
-        dvisd += dc1 * c1[i] + dc0 * c0[i];
-        const float dx1 = dc1 * visd * 2.f * c1[i] * (1.f - c1[i]), dx0 = dc0 * visd * 2.f * c0[i] * (1.f - c0[i]);
-        const float dmean = -(dx1 + dx0) * var[i];
-        const float dvar = dx1 * (hi - mean[i]) + dx0 * (lo - mean[i]);
-        dho[0][i] = dmean * (1.f - expf(-mean[i]));
-        dho[1][i] = dvar * (1.f - expf(-(var[i] - pp.var_bias)));
-      }
-      dho[2][0] = (dmix[0] - dmix[1]) * aw * (1.f - aw);
-      if (pp.use_vis) dho[3][0] = dvisd * visd * (1.f - visd);
+      Mix m;
+      float c0[2], c1[2];
+      ldv<2>(c.tr, R_MEAN, r, m.mean); ldv<2>(c.tr, R_VAR, r, m.var); ldv<2>(c.tr, R_C0, r, c0); ldv<2>(c.tr, R_C1, r, c1);
+      m.aw = c.tr.at(R_AW, r); m.visd = c.tr.at(R_VISD, r);
+      MixGrad dm = {};
+      bin_bwd(m, c.tr.at(R_TLO, r), c.tr.at(R_THI, r), c0, c1, 2.f * dhitn * mask, 2.f * dvisn * mask, dm);
+      mix_bwd(m, dm, pp.var_bias, pp.use_vis, dho);
     }
     // dist decoder heads
     for (int hd = 0; hd < c.n_heads; ++hd) {
-      const float* Wh = W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
       stv<2>(c.gr, G_DD2 + 2 * hd, r, dho[hd]);
-      float h2[32], dz1[32], h1[32], dz0[32], t[32];
+      float h2[32], h1[32];
       ldv<32>(c.tr, R_H2 + 32 * hd, r, h2);
-      for (int k = 0; k < 32; ++k) dz1[k] = (Wh[lay::DD_L2_W + k] * dho[hd][0] + Wh[lay::DD_L2_W + 32 + k] * dho[hd][1]) * elu_g(h2[k]);
-      stv<32>(c.gr, G_DD1 + 32 * hd, r, dz1);
-      lin_t<32, 32>(Wh + lay::DD_L1_W, dz1, dz0);
       ldv<32>(c.tr, R_H1 + 32 * hd, r, h1);
-      for (int k = 0; k < 32; ++k) dz0[k] *= elu_g(h1[k]);
-      stv<32>(c.gr, G_DD0 + 32 * hd, r, dz0);
-      lin_t<32, 32>(Wh + lay::DD_L0_W, dz0, t);
-      for (int k = 0; k < 32; ++k) drf[k] += t[k];
+      head_bwd(W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE, nullptr, h1, h2, dho[hd], drf, nullptr, &c.gr, r, hd);
     }
     for (int hd = c.n_heads; hd < 4; ++hd) {   // unused head: zero rows for the GEMMs
       float z[32];
@@ -1050,108 +1055,42 @@ typedef NrSelfParams SelfCtx;   // include/neuray_b200.h
 NR_HD void self_hit_prob_ray(const SelfCtx& c, long long ray) {
   const int dn = c.dn, fh = c.fh, fw = c.fw, n_heads = c.use_vis ? 4 : 3;
   const float* __restrict__ W = c.w_point;
-  // bilinear sample, border clamp (interpolate_feats, ops.py:14-34; align_corners when the map is full resolution)
-  const float x = c.coords[2 * ray], y = c.coords[2 * ray + 1];
-  const bool al = (fh == c.h && fw == c.w);
-  const float gx = x / float(c.w - 1) * 2.f - 1.f, gy = y / float(c.h - 1) * 2.f - 1.f;
-  float fx = al ? (gx + 1.f) / 2.f * float(fw - 1) : ((gx + 1.f) * float(fw) - 1.f) / 2.f;
-  float fy = al ? (gy + 1.f) / 2.f * float(fh - 1) : ((gy + 1.f) * float(fh) - 1.f) / 2.f;
-  fx = fminf(fmaxf(fx, 0.f), float(fw - 1)); fy = fminf(fmaxf(fy, 0.f), float(fh - 1));
-  const float x0f = floorf(fx), y0f = floorf(fy);
-  const int x0 = int(x0f), y0 = int(y0f);
-  const int x1 = x0 + 1 < fw ? x0 + 1 : fw - 1, y1 = y0 + 1 < fh ? y0 + 1 : fh - 1;
-  const float we = fx - x0f, ww = (x0f + 1.f) - fx, ws = fy - y0f, wn = (y0f + 1.f) - fy;
-  const float tw[4] = {ww * wn, we * wn, ww * ws, we * ws};
-  const int to[4] = {y0 * fw + x0, y0 * fw + x1, y1 * fw + x0, y1 * fw + x1};
+  const Taps tap = border_taps(c.coords[2 * ray], c.coords[2 * ray + 1], c.h, c.w, fh, fw, fh == c.h && fw == c.w);
   float rf[32];
-  for (int k = 0; k < 32; ++k) {
-    const float* m = c.map + (size_t)k * fh * fw;
-    rf[k] = m[to[0]] * tw[0] + m[to[1]] * tw[1] + m[to[2]] * tw[2] + m[to[3]] * tw[3];
-  }
+  for (int k = 0; k < 32; ++k) rf[k] = bilinear(c.map + (size_t)k * fh * fw, fw, tap);
   float h1[4][32], h2[4][32], ho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
-  for (int hd = 0; hd < n_heads; ++hd) {
-    const float* Wh = W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
-    lin<32, 32>(Wh + lay::DD_L0_W, Wh + lay::DD_L0_B, rf, h1[hd]);
-    for (int k = 0; k < 32; ++k) h1[hd][k] = elu_f(h1[hd][k]);
-    lin<32, 32>(Wh + lay::DD_L1_W, Wh + lay::DD_L1_B, h1[hd], h2[hd]);
-    for (int k = 0; k < 32; ++k) h2[hd][k] = elu_f(h2[hd][k]);
-    for (int o = 0; o < 2; ++o) {
-      float a = Wh[lay::DD_L2_B + o];
-      for (int k = 0; k < 32; ++k) a = fmaf(Wh[lay::DD_L2_W + o * 32 + k], h2[hd][k], a);
-      ho[hd][o] = a;
-    }
-  }
-  float mean[2], var[2];
-  for (int i = 0; i < 2; ++i) { mean[i] = softplus_f(ho[0][i]); var[i] = softplus_f(ho[1][i]) + c.var_bias; }
-  const float aw = sigm(ho[2][0]);
-  const float visd = c.use_vis ? sigm(ho[3][0]) : 1.f;
+  for (int hd = 0; hd < n_heads; ++hd) head_fwd(W + lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE, rf, h1[hd], h2[hd], ho[hd], nullptr, 0, 0);
+  const Mix m = mix_fwd(ho, c.var_bias, c.use_vis);
   // bin edges in normalised inverse depth (get_near_far_points, is_ref=False: midpoints, half intervals at the ends)
   const float a = -1.f / c.depth_range[0], b = -1.f / c.depth_range[1];
   const float* qd = c.que_depth + ray * dn;
   auto tn = [&](int s) { return (-1.f / fmaxf(qd[s], 1e-5f) - a) / (b - a); };
-  float dmean[2] = {0.f, 0.f}, dvar[2] = {0.f, 0.f}, dmix[2] = {0.f, 0.f}, dvisd = 0.f;
+  MixGrad dm = {};
   for (int s = 0; s < dn; ++s) {
     const float t = tn(s);
     const float lo = s == 0 ? t - (tn(1) - t) * 0.5f : (tn(s - 1) + t) * 0.5f;
     const float hi = s == dn - 1 ? t + 1e6f * 0.5f : (t + tn(s + 1)) * 0.5f;
-    float hit = 0.f, c0[2], c1[2];
-    for (int i = 0; i < 2; ++i) {
-      c0[i] = sigm(2.f * (lo - mean[i]) * var[i]);
-      c1[i] = sigm(2.f * (hi - mean[i]) * var[i]);
-      hit += (c1[i] - c0[i]) * visd * (i == 0 ? aw : 1.f - aw);
-    }
+    float c0[2], c1[2], hit, visb;
+    bin_fwd(m, lo, hi, c0, c1, hit, visb);
     c.hit[ray * dn + s] = hit;
-    if (c.d_hit != nullptr) {
-      const float dh = c.d_hit[ray * dn + s];
-      for (int i = 0; i < 2; ++i) {
-        const float mix = i == 0 ? aw : 1.f - aw;
-        const float dc = dh * mix;                                  // wrt c1*visd; -dc wrt c0*visd
-        dmix[i] += dh * (c1[i] - c0[i]) * visd;
-        dvisd += dc * (c1[i] - c0[i]);
-        const float dx1 = dc * visd * 2.f * c1[i] * (1.f - c1[i]), dx0 = -dc * visd * 2.f * c0[i] * (1.f - c0[i]);
-        dmean[i] -= (dx1 + dx0) * var[i];
-        dvar[i] += dx1 * (hi - mean[i]) + dx0 * (lo - mean[i]);
-      }
-    }
+    if (c.d_hit != nullptr) bin_bwd(m, lo, hi, c0, c1, c.d_hit[ray * dn + s], 0.f, dm);
   }
   if (c.d_hit == nullptr) return;
-  float dho[4][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
-  for (int i = 0; i < 2; ++i) {
-    dho[0][i] = dmean[i] * (1.f - expf(-mean[i]));
-    dho[1][i] = dvar[i] * (1.f - expf(-(var[i] - c.var_bias)));
-  }
-  dho[2][0] = (dmix[0] - dmix[1]) * aw * (1.f - aw);
-  if (c.use_vis) dho[3][0] = dvisd * visd * (1.f - visd);
+  float dho[4][2];
+  mix_bwd(m, dm, c.var_bias, c.use_vis, dho);
   float drf[32];
   for (int k = 0; k < 32; ++k) drf[k] = 0.f;
   for (int hd = 0; hd < n_heads; ++hd) {
     const int base = lay::DD_HEAD + hd * lay::DD_HEAD_STRIDE;
-    const float* Wh = W + base;
-    float* dWh = c.d_w_point + base;
-    float dz1[32], dz0[32], t[32];
-    for (int o = 0; o < 2; ++o) {
-      atomic_add(dWh + lay::DD_L2_B + o, dho[hd][o]);
-      for (int k = 0; k < 32; ++k) atomic_add(dWh + lay::DD_L2_W + o * 32 + k, dho[hd][o] * h2[hd][k]);
-    }
-    for (int k = 0; k < 32; ++k) dz1[k] = (Wh[lay::DD_L2_W + k] * dho[hd][0] + Wh[lay::DD_L2_W + 32 + k] * dho[hd][1]) * elu_g(h2[hd][k]);
-    lin_t<32, 32>(Wh + lay::DD_L1_W, dz1, dz0);
-    for (int k = 0; k < 32; ++k) dz0[k] *= elu_g(h1[hd][k]);
-    for (int j = 0; j < 32; ++j) {
-      atomic_add(dWh + lay::DD_L1_B + j, dz1[j]);
-      atomic_add(dWh + lay::DD_L0_B + j, dz0[j]);
-      for (int i = 0; i < 32; ++i) {                                  // WT[in][out]
-        atomic_add(dWh + lay::DD_L1_W + i * 32 + j, h1[hd][i] * dz1[j]);
-        atomic_add(dWh + lay::DD_L0_W + i * 32 + j, rf[i] * dz0[j]);
-      }
-    }
-    lin_t<32, 32>(Wh + lay::DD_L0_W, dz0, t);
-    for (int k = 0; k < 32; ++k) drf[k] += t[k];
+    head_bwd(W + base, rf, h1[hd], h2[hd], dho[hd], drf, c.d_w_point + base, nullptr, 0, 0);
   }
-  if (c.d_map != nullptr)
+  if (c.d_map != nullptr) {
+    const int off[4] = {tap.y0 * fw + tap.x0, tap.y0 * fw + tap.x1, tap.y1 * fw + tap.x0, tap.y1 * fw + tap.x1};
     for (int k = 0; k < 32; ++k) {
-      float* m = c.d_map + (size_t)k * fh * fw;
-      for (int q = 0; q < 4; ++q) atomic_add(m + to[q], drf[k] * tw[q]);
+      float* dmap = c.d_map + (size_t)k * fh * fw;
+      for (int q = 0; q < 4; ++q) atomic_add(dmap + off[q], drf[k] * tap.w[q]);
     }
+  }
 }
 
 }  // namespace tr
