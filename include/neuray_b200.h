@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 9
+#define NR_ABI_VERSION 10
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -94,6 +94,11 @@ typedef struct NrPassWeights {
  * kernel per buffer set on `stream`; `w` is a HOST struct of device pointers. */
 int nr_pack_weights(const NrPassWeights* w, float* w_point, float* w_ray, float* w_tc, void* stream);
 
+/* The tensor-core buffer of the point kernel's TF32 mode (nr_render_pass_fwd_tf32, nr_point_kernel_tf32): w_tc
+ * [NrTcLayout.total] in the same layout, each weight rounded to the nearest tf32 value (ties away from zero) in its hi
+ * slot, the lo slots zero.  The TF32 mode reads w_point and w_ray from nr_pack_weights as usual. */
+int nr_pack_weights_tf32(const NrPassWeights* w, float* w_tc, void* stream);
+
 /* ---- per-frame packing ---------------------------------------------------------------------------------- */
 
 /* que_cam [24] (NrPassParams.que_cam) and view_params [rfn,20] (NrPassParams.view_params) from the reference's camera
@@ -156,6 +161,12 @@ typedef struct NrPassParams {
  * following sample_fine_depth.  Two kernels: point kernel (per point x view) and ray kernel (per ray). */
 int nr_render_pass_fwd(const NrPassParams* p, void* stream);
 
+/* The same pass with the point kernel in TF32 mode: one tensor-core pass per product (3xTF32 issues three) on operands
+ * rounded to nearest, p->w_tc from nr_pack_weights_tf32 -- the arithmetic torch 1.7 - 1.11 used for nn.Linear on
+ * Ampere and later GPUs by default (~1e-3 relative per layer).  The ray kernel is the same as in nr_render_pass_fwd.
+ * nr_render_pass_bwd recomputes a pass in fp32, so a pass whose gradient is wanted runs nr_render_pass_fwd. */
+int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream);
+
 /* Direct rendering of the same pass (reference renderer.py:85-125, 181-185 and sph_solver.py, cfg use_dr_prediction),
  * forward only.  Enqueue it after nr_render_pass_fwd of the same NrPassParams: it reads the pass' inputs and, with
  * use_nr_color, the NR colours of its point record.  Per point: the per-view alpha logits of the active pass' dist decoder
@@ -175,6 +186,7 @@ int nr_direct_render(const NrPassParams* p, const NrDrParams* d, void* stream);
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);
+int nr_point_kernel_tf32(const NrPassParams* p, void* stream);   /* TF32 mode, as in nr_render_pass_fwd_tf32 */
 int nr_ray_kernel(const NrPassParams* p, void* stream);
 
 /* Stage-level debug tap of the point kernel: per (view, point) rows of

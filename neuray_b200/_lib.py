@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -72,11 +72,14 @@ SIGNATURES = {
     "nr_weight_layout": (C.c_int, [C.POINTER(NrWeightLayout)]),
     "nr_tc_layout": (C.c_int, [C.POINTER(NrTcLayout)]),
     "nr_pack_weights": (C.c_int, [C.POINTER(NrPassWeights), _vp, _vp, _vp, _vp]),
+    "nr_pack_weights_tf32": (C.c_int, [C.POINTER(NrPassWeights), _vp, _vp]),
     "nr_camera_blocks": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "nr_pack_feature_maps": (C.c_int, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "nr_render_pass_fwd": (C.c_int, [C.POINTER(NrPassParams), _vp]),
+    "nr_render_pass_fwd_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_direct_render": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrDrParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
+    "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_debug": (C.c_int, [C.POINTER(NrPassParams), _vp, _vp]),
     "nr_point_kernel_timing": (C.c_int, [C.POINTER(NrPassParams), _vp, _vp]),

@@ -230,7 +230,7 @@ __global__ void fine_depth_kernel(const float* __restrict__ depth, const float* 
 }  // namespace ops
 
 // implemented in nr_point_kernel.cu / nr_ray_kernel.cu
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, cudaStream_t stream);
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, bool tf32, cudaStream_t stream);
 int launch_ray_kernel(const NrPassParams* p, cudaStream_t stream);
 
 static thread_local char g_err[512] = "";
@@ -294,18 +294,24 @@ int nr_pack_feature_maps(const float* ray_feats, const float* img_feats, const f
   return NR_OK;
 }
 
-int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, (cudaStream_t)stream); }
+int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, false, (cudaStream_t)stream); }
+int nr_point_kernel_tf32(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, true, (cudaStream_t)stream); }
 int nr_point_kernel_debug(const NrPassParams* p, float* dbg, void* stream) {
   NR_CHECK_ARG(dbg != nullptr, "dbg");
-  return launch_point_kernel(p, dbg, nullptr, (cudaStream_t)stream);
+  return launch_point_kernel(p, dbg, nullptr, false, (cudaStream_t)stream);
 }
 int nr_point_kernel_timing(const NrPassParams* p, long long* timing, void* stream) {
   NR_CHECK_ARG(timing != nullptr && p != nullptr && p->w_tc != nullptr, "timing buffer / tensor-core weights required");
-  return launch_point_kernel(p, nullptr, timing, (cudaStream_t)stream);
+  return launch_point_kernel(p, nullptr, timing, false, (cudaStream_t)stream);
 }
 int nr_ray_kernel(const NrPassParams* p, void* stream) { return launch_ray_kernel(p, (cudaStream_t)stream); }
 int nr_render_pass_fwd(const NrPassParams* p, void* stream) {
-  const int rc = launch_point_kernel(p, nullptr, nullptr, (cudaStream_t)stream);
+  const int rc = launch_point_kernel(p, nullptr, nullptr, false, (cudaStream_t)stream);
+  if (rc != NR_OK) return rc;
+  return launch_ray_kernel(p, (cudaStream_t)stream);
+}
+int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream) {
+  const int rc = launch_point_kernel(p, nullptr, nullptr, true, (cudaStream_t)stream);
   if (rc != NR_OK) return rc;
   return launch_ray_kernel(p, (cudaStream_t)stream);
 }

@@ -3,6 +3,8 @@
 //
 //   nr_pack_weights   parameters of one pass in PyTorch's [out][in] layout -> the three flat buffers the kernels read
 //                     (w_point, w_ray: NrWeightLayout; w_tc: NrTcLayout = hi/lo tf32 parts in K-major SWIZZLE_128B tiles)
+//   nr_pack_weights_tf32  the same pass -> w_tc of the point kernel's TF32 mode: the same layout, each weight rounded
+//                     to the nearest tf32 value in its hi slot, the lo slots zero
 //   nr_camera_blocks  poses / intrinsics / depth ranges -> que_cam [24] and view_params [rfn,20]
 //
 // Both are single launches with no host synchronisation and no library-side state.
@@ -32,14 +34,26 @@ struct Out {
   float* wt;
 };
 
-// element (row n, column k) of the tensor-core tile at `off` with layout t: slab k/32, swizzled inside
+// element (row n, column k) of the tensor-core tile at `off` with layout t: slab k/32, swizzled inside.  TF32: rna(v) in
+// the hi slot and nothing in the lo slot (the TF32 point kernel reads only hi)
+template <bool TF32>
 __device__ __forceinline__ void put_tc(float* wt, int off, tcl::Tile t, int n, int k, float v) {
   const int pos = off + (k >> 5) * t.slab + tc::sw128_index(n, k & 31);
-  const float hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-  wt[pos + t.hi] = hi;
-  wt[pos + t.lo] = v - hi;
+  if constexpr (TF32) {
+    wt[pos + t.hi] = __uint_as_float(tc::tf32_rna(v));
+  } else {
+    const float hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
+    wt[pos + t.hi] = hi;
+    wt[pos + t.lo] = v - hi;
+  }
+}
+// an entry of w_point / w_ray (the TF32 pack writes neither)
+template <bool TF32>
+__device__ __forceinline__ void put_w(float* buf, int i, float v) {
+  if constexpr (!TF32) buf[i] = v;
 }
 
+template <bool TF32>
 __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
   const int job = blockIdx.x;
   const Job J = jobs.j[job];
@@ -56,7 +70,7 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
       const int r = e >> 5, k = e & 31;
       double acc = 0.0;
       for (int j = 0; j < 32; ++j) acc = fma(double(nf0[r * 32 + j]), double(pe1[j * 32 + k]), acc);
-      put_tc(wt, tcl::PE1, tcl::PE1_L, 32 + r, k, float(acc));
+      put_tc<TF32>(wt, tcl::PE1, tcl::PE1_L, 32 + r, k, float(acc));
     }
     return;
   }
@@ -67,58 +81,58 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
     if (job < 12) {
       const int h = job / 3, l = job - 3 * h;
       const int base = lay::DD_HEAD + h * lay::DD_HEAD_STRIDE;
-      if (l == 0) { wp[base + lay::DD_L0_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L0, o, i, v); }
-      else if (l == 1) { wp[base + lay::DD_L1_W + i * 32 + o] = v; put_tc(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L1, o, i, v); }
-      else wp[base + lay::DD_L2_W + o * 32 + i] = v;
+      if (l == 0) { put_w<TF32>(wp, base + lay::DD_L0_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L0, o, i, v); }
+      else if (l == 1) { put_w<TF32>(wp, base + lay::DD_L1_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::HEAD0 + h * tcl::STAGE, tcl::HEAD_L1, o, i, v); }
+      else put_w<TF32>(wp, base + lay::DD_L2_W + o * 32 + i, v);
       continue;
     }
     switch (job) {
-      case J_PE0: wp[lay::GRP_B + lay::PE0_W + i * 32 + o] = v; put_tc(wt, tcl::PE0, tcl::PE0_L, o, i, v); break;
-      case J_PE1: wp[lay::GRP_B + lay::PE1_W + i * 32 + o] = v; put_tc(wt, tcl::PE1, tcl::PE1_L, o, i, v); break;
-      case J_RD0: wp[lay::GRP_B + lay::RD0_W + i * 16 + o] = v; break;
-      case J_RD1: wp[lay::GRP_B + lay::RD1_W + i * 36 + o] = v; put_tc(wt, tcl::RD1, tcl::RD1_L, o, i, v); break;
-      case J_NF0: wp[lay::GRP_B + lay::NF0_W + i * 8 + o] = v; break;
-      case J_NF1: wp[lay::GRP_B + lay::NF1_W + i] = v; break;
+      case J_PE0: put_w<TF32>(wp, lay::GRP_B + lay::PE0_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::PE0, tcl::PE0_L, o, i, v); break;
+      case J_PE1: put_w<TF32>(wp, lay::GRP_B + lay::PE1_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::PE1, tcl::PE1_L, o, i, v); break;
+      case J_RD0: put_w<TF32>(wp, lay::GRP_B + lay::RD0_W + i * 16 + o, v); break;
+      case J_RD1: put_w<TF32>(wp, lay::GRP_B + lay::RD1_W + i * 36 + o, v); put_tc<TF32>(wt, tcl::RD1, tcl::RD1_L, o, i, v); break;
+      case J_NF0: put_w<TF32>(wp, lay::GRP_B + lay::NF0_W + i * 8 + o, v); break;
+      case J_NF1: put_w<TF32>(wp, lay::GRP_B + lay::NF1_W + i, v); break;
       case J_B0: {   // base_fc.0 [64,207] = [view-pooled 140 | rgb_feat 35 | neuray_feat 32]
         if (i < 140) {
-          wp[lay::HOIST_W + i * 64 + o] = v;
+          put_w<TF32>(wp, lay::HOIST_W + i * 64 + o, v);
           const int s = i / 35, f = i - 35 * s, r = f >> 3, q = f & 7;        // stat, feature -> K = 32 r + 8 s + q
-          put_tc(wt, tcl::HST, tcl::HST_L, o, 32 * r + 8 * s + q, v);
+          put_tc<TF32>(wt, tcl::HST, tcl::HST_L, o, 32 * r + 8 * s + q, v);
         } else {
-          wp[lay::BASE0_W + (i - 140) * 64 + o] = v;
+          put_w<TF32>(wp, lay::BASE0_W + (i - 140) * 64 + o, v);
           const int k = i < 175 ? i - 140 : 40 + (i - 175);                    // rgb_feat 35 | bias | 4 zeros | neuray_feat 32
-          put_tc(wt, tcl::B0, tcl::B0_L, o, k, v);
+          put_tc<TF32>(wt, tcl::B0, tcl::B0_L, o, k, v);
         }
         break;
       }
-      case J_B1: wp[lay::BASE1_W + i * 32 + o] = v; put_tc(wt, tcl::B1, tcl::B1_L, o, i, v); break;
-      case J_V0: wp[lay::GRP_D1 + lay::VIS0_W + i * 32 + o] = v; put_tc(wt, tcl::V01, tcl::VIS0_L, o, i, v); break;
+      case J_B1: put_w<TF32>(wp, lay::BASE1_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::B1, tcl::B1_L, o, i, v); break;
+      case J_V0: put_w<TF32>(wp, lay::GRP_D1 + lay::VIS0_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::V01, tcl::VIS0_L, o, i, v); break;
       case J_V1:
-        if (o < 32) { wp[lay::GRP_D1 + lay::VIS1_W + i * 32 + o] = v; put_tc(wt, tcl::V01, tcl::VIS2_L, o, i, v); }
-        else wp[lay::GRP_D1 + lay::VIS1L_W + i] = v;
+        if (o < 32) { put_w<TF32>(wp, lay::GRP_D1 + lay::VIS1_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::V01, tcl::VIS2_L, o, i, v); }
+        else put_w<TF32>(wp, lay::GRP_D1 + lay::VIS1L_W + i, v);
         break;
-      case J_V20: wp[lay::GRP_D1 + lay::V20_W + i * 32 + o] = v; put_tc(wt, tcl::V2R, tcl::V20_L, o, i, v); break;
-      case J_V21: wp[lay::GRP_D1 + lay::V21_W + i] = v; break;
-      case J_C0: wp[lay::GRP_D1 + lay::RGB0_W + i * 16 + o] = v; put_tc(wt, tcl::V2R, tcl::RGB0_L, o, i, v); break;
-      case J_C1: wp[lay::GRP_D1 + lay::RGB1_W + i * 8 + o] = v; break;
-      case J_C2: wp[lay::GRP_D1 + lay::RGB2_W + i] = v; break;
+      case J_V20: put_w<TF32>(wp, lay::GRP_D1 + lay::V20_W + i * 32 + o, v); put_tc<TF32>(wt, tcl::V2R, tcl::V20_L, o, i, v); break;
+      case J_V21: put_w<TF32>(wp, lay::GRP_D1 + lay::V21_W + i, v); break;
+      case J_C0: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB0_W + i * 16 + o, v); put_tc<TF32>(wt, tcl::V2R, tcl::RGB0_L, o, i, v); break;
+      case J_C1: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB1_W + i * 8 + o, v); break;
+      case J_C2: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB2_W + i, v); break;
       case J_G0: {   // geometry_fc.0 [64,65] = [mean 32 | var 32 | mean weight]
-        wp[lay::GRP_D2 + lay::GEO0_W + i * 64 + o] = v;
+        put_w<TF32>(wp, lay::GRP_D2 + lay::GEO0_W + i * 64 + o, v);
         int k;
         if (i < 64) { const int s = i >> 5, f = i & 31, r = f >> 4, q = f & 15; k = 32 * r + 16 * s + q; }
         else k = 64;
-        put_tc(wt, tcl::G0, tcl::G0_L, o, k, v);
+        put_tc<TF32>(wt, tcl::G0, tcl::G0_L, o, k, v);
         break;
       }
-      case J_G1: wp[lay::GRP_D2 + lay::GEO1_W + i * 16 + o] = v; break;
-      case J_OG0: wr[lay::OG0_W + i * 16 + o] = v; break;
-      case J_OG1: wr[lay::OG1_W + i] = v; break;
-      case J_WQ: wr[lay::WQ + i * 16 + o] = v; break;
-      case J_WK: wr[lay::WK + i * 16 + o] = v; break;
-      case J_WV: wr[lay::WV + i * 16 + o] = v; break;
-      case J_WFC: wr[lay::WFC + i * 16 + o] = v; break;
-      case J_LNW: wr[lay::LN_W + e] = v; break;
-      case J_LNB: wr[lay::LN_B + e] = v; break;
+      case J_G1: put_w<TF32>(wp, lay::GRP_D2 + lay::GEO1_W + i * 16 + o, v); break;
+      case J_OG0: put_w<TF32>(wr, lay::OG0_W + i * 16 + o, v); break;
+      case J_OG1: put_w<TF32>(wr, lay::OG1_W + i, v); break;
+      case J_WQ: put_w<TF32>(wr, lay::WQ + i * 16 + o, v); break;
+      case J_WK: put_w<TF32>(wr, lay::WK + i * 16 + o, v); break;
+      case J_WV: put_w<TF32>(wr, lay::WV + i * 16 + o, v); break;
+      case J_WFC: put_w<TF32>(wr, lay::WFC + i * 16 + o, v); break;
+      case J_LNW: put_w<TF32>(wr, lay::LN_W + e, v); break;
+      case J_LNB: put_w<TF32>(wr, lay::LN_B + e, v); break;
       default: break;
     }
   }
@@ -129,29 +143,29 @@ __global__ void pack_weights_kernel(const Jobs jobs, const Out out) {
     if (job < 12) {
       const int h = job / 3, l = job - 3 * h;
       const int base = lay::DD_HEAD + h * lay::DD_HEAD_STRIDE;
-      wp[base + (l == 0 ? lay::DD_L0_B : l == 1 ? lay::DD_L1_B : lay::DD_L2_B) + o] = v;
+      put_w<TF32>(wp, base + (l == 0 ? lay::DD_L0_B : l == 1 ? lay::DD_L1_B : lay::DD_L2_B) + o, v);
       continue;
     }
     switch (job) {
-      case J_PE0: wp[lay::GRP_B + lay::PE0_B + o] = v; break;
-      case J_PE1: wp[lay::GRP_B + lay::PE1_B + o] = v; break;
-      case J_RD0: wp[lay::GRP_B + lay::RD0_B + o] = v; break;
-      case J_RD1: wp[lay::GRP_B + lay::RD1_B + o] = v; break;
-      case J_NF0: wp[lay::GRP_B + lay::NF0_B + o] = v; break;
-      case J_NF1: wp[lay::GRP_B + lay::NF1_B + o] = v; break;
-      case J_B0: wp[lay::HOIST_B + o] = v; put_tc(wt, tcl::B0, tcl::B0_L, o, 35, v); break;   // bias = column 35 (constant-1 input)
-      case J_B1: wp[lay::BASE1_B + o] = v; break;
-      case J_V0: wp[lay::GRP_D1 + lay::VIS0_B + o] = v; break;
-      case J_V1: wp[lay::GRP_D1 + (o < 32 ? lay::VIS1_B + o : lay::VIS1L_B)] = v; break;
-      case J_V20: wp[lay::GRP_D1 + lay::V20_B + o] = v; break;
-      case J_V21: wp[lay::GRP_D1 + lay::V21_B + o] = v; break;
-      case J_C0: wp[lay::GRP_D1 + lay::RGB0_B + o] = v; break;
-      case J_C1: wp[lay::GRP_D1 + lay::RGB1_B + o] = v; break;
-      case J_C2: wp[lay::GRP_D1 + lay::RGB2_B + o] = v; break;
-      case J_G0: wp[lay::GRP_D2 + lay::GEO0_B + o] = v; put_tc(wt, tcl::G0, tcl::G0_L, o, 65, v); break;   // bias = column 65
-      case J_G1: wp[lay::GRP_D2 + lay::GEO1_B + o] = v; break;
-      case J_OG0: wr[lay::OG0_B + o] = v; break;
-      case J_OG1: wr[lay::OG1_B + o] = v; break;
+      case J_PE0: put_w<TF32>(wp, lay::GRP_B + lay::PE0_B + o, v); break;
+      case J_PE1: put_w<TF32>(wp, lay::GRP_B + lay::PE1_B + o, v); break;
+      case J_RD0: put_w<TF32>(wp, lay::GRP_B + lay::RD0_B + o, v); break;
+      case J_RD1: put_w<TF32>(wp, lay::GRP_B + lay::RD1_B + o, v); break;
+      case J_NF0: put_w<TF32>(wp, lay::GRP_B + lay::NF0_B + o, v); break;
+      case J_NF1: put_w<TF32>(wp, lay::GRP_B + lay::NF1_B + o, v); break;
+      case J_B0: put_w<TF32>(wp, lay::HOIST_B + o, v); put_tc<TF32>(wt, tcl::B0, tcl::B0_L, o, 35, v); break;   // bias = column 35 (constant-1 input)
+      case J_B1: put_w<TF32>(wp, lay::BASE1_B + o, v); break;
+      case J_V0: put_w<TF32>(wp, lay::GRP_D1 + lay::VIS0_B + o, v); break;
+      case J_V1: put_w<TF32>(wp, lay::GRP_D1 + (o < 32 ? lay::VIS1_B + o : lay::VIS1L_B), v); break;
+      case J_V20: put_w<TF32>(wp, lay::GRP_D1 + lay::V20_B + o, v); break;
+      case J_V21: put_w<TF32>(wp, lay::GRP_D1 + lay::V21_B + o, v); break;
+      case J_C0: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB0_B + o, v); break;
+      case J_C1: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB1_B + o, v); break;
+      case J_C2: put_w<TF32>(wp, lay::GRP_D1 + lay::RGB2_B + o, v); break;
+      case J_G0: put_w<TF32>(wp, lay::GRP_D2 + lay::GEO0_B + o, v); put_tc<TF32>(wt, tcl::G0, tcl::G0_L, o, 65, v); break;   // bias = column 65
+      case J_G1: put_w<TF32>(wp, lay::GRP_D2 + lay::GEO1_B + o, v); break;
+      case J_OG0: put_w<TF32>(wr, lay::OG0_B + o, v); break;
+      case J_OG1: put_w<TF32>(wr, lay::OG1_B + o, v); break;
       default: break;
     }
   }
@@ -209,10 +223,8 @@ __global__ void camera_blocks_kernel(const float* __restrict__ que_pose, const f
 
 using namespace nr;
 
-extern "C" {
-
-int nr_pack_weights(const NrPassWeights* w, float* w_point, float* w_ray, float* w_tc, void* stream) {
-  NR_CHECK_ARG(w != nullptr && w_point != nullptr && w_ray != nullptr && w_tc != nullptr, "null pointer");
+// The job table of a pass, checked; tf32: only w_tc, for the TF32 point kernel
+static int pack_pass(const NrPassWeights* w, float* w_point, float* w_ray, float* w_tc, bool tf32, cudaStream_t s) {
   pack::Jobs jobs;
   auto set = [&](int j, const NrLinear& l, int n_out, int n_in) { jobs.j[j] = pack::Job{l.w, l.b, n_out, n_in}; };
   for (int h = 0; h < 4; ++h) {
@@ -253,13 +265,30 @@ int nr_pack_weights(const NrPassWeights* w, float* w_point, float* w_ray, float*
   jobs.j[pack::J_LNW] = pack::Job{w->layer_norm_w, nullptr, 16, 1};
   jobs.j[pack::J_LNB] = pack::Job{w->layer_norm_b, nullptr, 16, 1};
   jobs.j[pack::J_COMP] = pack::Job{w->neuray_fc[0].w, w->prob_embed[1].w, 8, 32};
-  cudaStream_t s = (cudaStream_t)stream;
+  if (tf32) {
+    cudaMemsetAsync(w_tc, 0, sizeof(float) * tcl::TOTAL, s);
+    pack::pack_weights_kernel<true><<<pack::NJOBS, 256, 0, s>>>(jobs, pack::Out{nullptr, nullptr, w_tc});
+    NR_CHECK_LAUNCH("pack_weights_tf32");
+    return NR_OK;
+  }
   cudaMemsetAsync(w_point, 0, sizeof(float) * lay::TOTAL_POINT, s);
   cudaMemsetAsync(w_ray, 0, sizeof(float) * lay::TOTAL_RAY, s);
   cudaMemsetAsync(w_tc, 0, sizeof(float) * tcl::TOTAL, s);
-  pack::pack_weights_kernel<<<pack::NJOBS, 256, 0, s>>>(jobs, pack::Out{w_point, w_ray, w_tc});
+  pack::pack_weights_kernel<false><<<pack::NJOBS, 256, 0, s>>>(jobs, pack::Out{w_point, w_ray, w_tc});
   NR_CHECK_LAUNCH("pack_weights");
   return NR_OK;
+}
+
+extern "C" {
+
+int nr_pack_weights(const NrPassWeights* w, float* w_point, float* w_ray, float* w_tc, void* stream) {
+  NR_CHECK_ARG(w != nullptr && w_point != nullptr && w_ray != nullptr && w_tc != nullptr, "null pointer");
+  return pack_pass(w, w_point, w_ray, w_tc, false, (cudaStream_t)stream);
+}
+
+int nr_pack_weights_tf32(const NrPassWeights* w, float* w_tc, void* stream) {
+  NR_CHECK_ARG(w != nullptr && w_tc != nullptr, "null pointer");
+  return pack_pass(w, nullptr, nullptr, w_tc, true, (cudaStream_t)stream);
 }
 
 int nr_camera_blocks(const float* que_pose, const float* que_K, const float* que_range, const float* ref_poses, const float* ref_Ks,

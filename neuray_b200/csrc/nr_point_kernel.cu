@@ -13,6 +13,8 @@
 //     stage_source; full/empty mbarriers, the "empty" barrier takes one arrival from thread 0 of each compute warp group
 //     once that warp group's consuming wgmma have completed (Ring: the compute threads' side)
 //   * where each layer's B sits inside its ring stage is a tcl::Tile (nr_common.cuh), shared with the weight packer
+//   * TF32 mode (point_kernel_tf32, inference): the same body with one tensor-core pass per product instead of three, A
+//     rounded to nearest where the 3xTF32 body splits it, B from nr_pack_weights_tf32 (rna(W) in the hi slots)
 #include <type_traits>
 
 #include "nr_common.cuh"
@@ -308,32 +310,39 @@ static int device_sms() {
 // The dynamic shared-memory opt-in is a per-device function attribute; it is set on every launch (a few hundred
 // nanoseconds against a kernel of milliseconds) so that the library keeps no per-process state: a process may render on
 // any number of devices from any number of threads.
-template <int G, bool DEBUG>
+// TF32: the TF32-mode kernel (release form only), else the 3xTF32 one
+template <int G, bool DEBUG, bool TF32>
 static int launch_pm3_inst(const pkt::KParams& kp, int grid, cudaStream_t stream) {
-  auto* fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
+  static_assert(!(TF32 && DEBUG), "the TF32 mode has no debug form");
+  void (*fn)(const pkt::KParams);
+  if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
+  else fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
   if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(pkt::pm3::SMEM_BYTES)) != cudaSuccess) {
     nr::set_error("point kernel: cannot opt in to %zu bytes of shared memory: %s", pkt::pm3::SMEM_BYTES, cudaGetErrorString(cudaGetLastError()));
     return NR_E_CUDA;
   }
   fn<<<grid, pkt::pm3::NTHR, pkt::pm3::SMEM_BYTES, stream>>>(kp);
-  NR_CHECK_LAUNCH("point_kernel_pm3");
+  NR_CHECK_LAUNCH(TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
   return NR_OK;
 }
 
 template <int G>
-static int launch_pm3(pkt::KParams kp, cudaStream_t stream) {
+static int launch_pm3(pkt::KParams kp, bool tf32, cudaStream_t stream) {
   constexpr int PB = 4 * (32 / G);       // points per 128-row block: 32 / G per warp (G not a power of two leaves 32 % G lanes idle)
   const long long N = (long long)kp.p.rn * kp.p.dn;
   kp.P = PB;
   kp.n_tiles = int((N + PB - 1) / PB);
   const int sms = device_sms();
   const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
-  return (kp.dbg || kp.timing) ? launch_pm3_inst<G, true>(kp, grid, stream) : launch_pm3_inst<G, false>(kp, grid, stream);
+  if (tf32) return launch_pm3_inst<G, false, true>(kp, grid, stream);
+  return (kp.dbg || kp.timing) ? launch_pm3_inst<G, true, false>(kp, grid, stream) : launch_pm3_inst<G, false, false>(kp, grid, stream);
 }
 
-// `timing`: optional clock64() stamps at the phase boundaries (nr_point_kernel_timing), passed per call
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, cudaStream_t stream) {
+// `timing`: optional clock64() stamps at the phase boundaries (nr_point_kernel_timing), passed per call.  tf32: the TF32
+// mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr, "params");
+  NR_CHECK_ARG(!tf32 || (dbg == nullptr && timing == nullptr), "the TF32 point kernel has no debug tap or phase stamps");
   NR_CHECK_ARG(p->coords && p->que_depth && p->que_cam && p->feat && p->rgb && p->view_params && p->w_point && p->point_rec,
                "null device pointer");
   NR_CHECK_ARG(p->w_tc != nullptr, "w_tc (tensor-core weight buffer, nr_pack_weights) is required");
@@ -350,13 +359,13 @@ int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, cu
   kp.timing = timing;
   kp.n_heads = p->use_vis ? 4 : 3;
   // lanes per point: the smallest group size that holds the views and wastes the fewest of a warp's 32 lanes
-  if (p->rfn <= 4) return launch_pm3<4>(kp, stream);
-  if (p->rfn == 5) return launch_pm3<5>(kp, stream);      // 6 points per warp (30 lanes) instead of 4 groups of 8
-  if (p->rfn == 6) return launch_pm3<6>(kp, stream);      // 5 points per warp
-  if (p->rfn <= 8) return launch_pm3<8>(kp, stream);
-  if (p->rfn <= 10) return launch_pm3<10>(kp, stream);    // 3 points per warp instead of 2 groups of 16 (cfg4: 10 views)
-  if (p->rfn <= 16) return launch_pm3<16>(kp, stream);
-  return launch_pm3<32>(kp, stream);
+  if (p->rfn <= 4) return launch_pm3<4>(kp, tf32, stream);
+  if (p->rfn == 5) return launch_pm3<5>(kp, tf32, stream);      // 6 points per warp (30 lanes) instead of 4 groups of 8
+  if (p->rfn == 6) return launch_pm3<6>(kp, tf32, stream);      // 5 points per warp
+  if (p->rfn <= 8) return launch_pm3<8>(kp, tf32, stream);
+  if (p->rfn <= 10) return launch_pm3<10>(kp, tf32, stream);    // 3 points per warp instead of 2 groups of 16 (cfg4: 10 views)
+  if (p->rfn <= 16) return launch_pm3<16>(kp, tf32, stream);
+  return launch_pm3<32>(kp, tf32, stream);
 }
 
 }  // namespace nr

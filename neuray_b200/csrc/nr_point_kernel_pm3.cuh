@@ -11,7 +11,7 @@
 //     apart.  rgb_fc.1/.2 and the colour blend run in warp group 1 only, geometry_fc.2 in warp group 0 only, each from the
 //     whole row in the tile.
 //   * MMAs: warp group c issues the m64 wgmma of rows 64c .. 64c + 63 of every layer, each layer as one 3xTF32 batch
-//     (mma_batch).  Every per-view layer runs in the accumulator fragment of the warp group that issues it, for its own
+//     (mma_batch; the TF32 mode, point_kernel_tf32, issues the hi*hi pass alone: NP = 1).  Every per-view layer runs in the accumulator fragment of the warp group that issues it, for its own
 //     64 rows: the dist-decoder heads (run_head), the front hit/vis .. base_fc.0 (in the kernel body) and the tail
 //     base_fc.2 .. rgb_fc.0 (run_chain).  Nothing in them is pooled or needs the row-owner layout; A comes from registers
 //     after each stretch's first layer, row sums run over the 4 lanes that hold a row, and the results go to the row
@@ -106,18 +106,28 @@ __host__ __device__ constexpr int rf_slab_index(int r, int c) { return (r >> 6) 
 static_assert(rf_slab_index(63, 31) < 2048 && rf_slab_index(64, 0) == 2048 && rf_slab_index(127, 31) < 4096 &&
                   tc::act_index(64, 64) - RF_SLAB == 2048, "rgb_feat: each warp group's rows in its own half of slab 2");
 
-// ---- per-point layers: [points x K] x [K x 64] on warp-level mma.sync, 3xTF32 ----
+// ---- passes per product: NP = 3 (3xTF32, fp32 accuracy) or 1 (TF32 mode: the hi*hi pass alone) ----
+// An A operand value -> its hi part and, for NP = 3, its lo part.  NP = 1 rounds to nearest (tc::tf32_rna) and leaves
+// lo unwritten: no pass reads it.
+template <int NP>
+__device__ __forceinline__ void split(float x, uint32_t& hi, uint32_t& lo) {
+  static_assert(NP == 1 || NP == 3, "passes per product");
+  if constexpr (NP == 3) tc::split_tf32(x, hi, lo);
+  else hi = tc::tf32_rna(x);
+}
+
+// ---- per-point layers: [points x K] x [K x 64] on warp-level mma.sync, NP passes ----
 // Compute warp w (of 8) computes outputs 8w .. 8w + 7 for all PB points of the tile: MT m16 tiles of points, and one
-// accumulator per 3xTF32 pass (hi*hi, lo*hi, hi*lo) so that the three MMAs of a K step do not wait for each other.
-template <int PB>
+// accumulator per pass (hi*hi, lo*hi, hi*lo) so that the MMAs of a K step do not wait for each other.
+template <int PB, int NP>
 struct PtAcc {
   static constexpr int MT = (PB + 15) / 16;
-  float d[MT][3][4];
+  float d[MT][NP][4];
 };
 // acc += op[points][kcol + k] * W[8w + n][k], k < 8 KS: B from a weight ring stage `w` that holds one K32 slab of a 64-row
 // tile with layout L (K steps 0 .. KS - 1).  Operand rows at or past PB read as 0.
-template <int PB, int KS>
-__device__ __forceinline__ void point_mma(PtAcc<PB>& acc, const float* __restrict__ op, int kcol, const float* __restrict__ w, tcl::Tile L, int warp,
+template <int PB, int KS, int NP>
+__device__ __forceinline__ void point_mma(PtAcc<PB, NP>& acc, const float* __restrict__ op, int kcol, const float* __restrict__ w, tcl::Tile L, int warp,
                                           int lane) {
   const int g = lane >> 2, t = lane & 3;
   const float* __restrict__ bw = w + L.hi + warp * 256 + g * 32 + t;      // tc::sw128_index(8 warp + g, 8 j + t) = bw[((2j) ^ g) << 2]
@@ -125,37 +135,46 @@ __device__ __forceinline__ void point_mma(PtAcc<PB>& acc, const float* __restric
 #pragma unroll
   for (int j = 0; j < KS; ++j) {
     const uint32_t bh[2] = {__float_as_uint(bw[((2 * j) ^ g) << 2]), __float_as_uint(bw[((2 * j + 1) ^ g) << 2])};
-    const uint32_t bl[2] = {__float_as_uint(bw[L.lo - L.hi + (((2 * j) ^ g) << 2)]), __float_as_uint(bw[L.lo - L.hi + (((2 * j + 1) ^ g) << 2)])};
+    uint32_t bl[2];
+    if constexpr (NP == 3) {
+      bl[0] = __float_as_uint(bw[L.lo - L.hi + (((2 * j) ^ g) << 2)]);
+      bl[1] = __float_as_uint(bw[L.lo - L.hi + (((2 * j + 1) ^ g) << 2)]);
+    }
 #pragma unroll
-    for (int m = 0; m < PtAcc<PB>::MT; ++m) {
+    for (int m = 0; m < PtAcc<PB, NP>::MT; ++m) {
       const bool ok0 = 16 * m + 8 <= PB || 16 * m + g < PB, ok1 = 16 * m + 16 <= PB || 16 * m + 8 + g < PB;
       const float* __restrict__ a = aw + 16 * m * OP_ROW + 8 * j;
       const float x[4] = {ok0 ? a[0] : 0.f, ok1 ? a[8 * OP_ROW] : 0.f, ok0 ? a[4] : 0.f, ok1 ? a[8 * OP_ROW + 4] : 0.f};
       uint32_t ah[4], al[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) tc::split_tf32(x[i], ah[i], al[i]);
+      for (int i = 0; i < 4; ++i) split<NP>(x[i], ah[i], al[i]);
       tc::mma_tf32_m16n8k8(acc.d[m][0], ah, bh);
-      tc::mma_tf32_m16n8k8(acc.d[m][1], al, bh);
-      tc::mma_tf32_m16n8k8(acc.d[m][2], ah, bl);
+      if constexpr (NP == 3) {
+        tc::mma_tf32_m16n8k8(acc.d[m][1], al, bh);
+        tc::mma_tf32_m16n8k8(acc.d[m][2], ah, bl);
+      }
     }
   }
 }
 // the accumulated outputs -> pt[point][8w .. 8w + 7] (points < PB)
-template <int PB>
-__device__ __forceinline__ void point_store(const PtAcc<PB>& acc, float* __restrict__ pt, int warp, int lane) {
+template <int PB, int NP>
+__device__ __forceinline__ void point_store(const PtAcc<PB, NP>& acc, float* __restrict__ pt, int warp, int lane) {
   const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-  for (int m = 0; m < PtAcc<PB>::MT; ++m) {
+  for (int m = 0; m < PtAcc<PB, NP>::MT; ++m) {
     float o[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) o[i] = acc.d[m][0][i] + (acc.d[m][1][i] + acc.d[m][2][i]);
+    for (int i = 0; i < 4; ++i) {
+      if constexpr (NP == 3) o[i] = acc.d[m][0][i] + (acc.d[m][1][i] + acc.d[m][2][i]);
+      else o[i] = acc.d[m][0][i];
+    }
     float* __restrict__ p = pt + (16 * m + g) * PT_ROW + 8 * warp + 2 * t;
     if (16 * m + 8 <= PB || 16 * m + g < PB) *reinterpret_cast<float2*>(p) = make_float2(o[0], o[1]);
     if (16 * m + 16 <= PB || 16 * m + 8 + g < PB) *reinterpret_cast<float2*>(p + 8 * PT_ROW) = make_float2(o[2], o[3]);
   }
 }
 
-// ---- tensor-core layers: one 3xTF32 wgmma batch each ----
+// ---- tensor-core layers: one wgmma batch of NP passes each ----
 // A operand of a batch from the activation tile: K step c at column col + 8c, its lo part lo_off columns further, rows
 // 64 wg .. 64 wg + 63
 struct TileA {
@@ -166,16 +185,16 @@ struct TileA {
   __device__ uint64_t operator()(int c, bool lo) const { return tc::act_desc(act_addr, col + 8 * c + (lo ? lo_off : 0), wg); }
 };
 __device__ __forceinline__ TileA tile_a(const Blk& b, int col, int lo_off) { return TileA{b.act_addr, b.wg, col, lo_off}; }
-// A from registers (tc::wgmma_tf32_ra): K step c from h[c] / l[c].  The K steps a batch reads stay pinned until it has
-// completed.
-template <int KA>
+// A from registers (tc::wgmma_tf32_ra): K step c from h[c] / l[c] (l only for NP = 3).  The K steps a batch reads stay
+// pinned until it has completed.
+template <int KA, int NP>
 struct RegA {
   uint32_t (&h)[KA][4];
   uint32_t (&l)[KA][4];
   template <int KS>
   __device__ void pin() const {
     tc::wgmma_fence_operand<KS>(h);
-    tc::wgmma_fence_operand<KS>(l);
+    if constexpr (NP == 3) tc::wgmma_fence_operand<KS>(l);
   }
   __device__ const uint32_t (&operator()(int c, bool lo) const)[4] { return lo ? l[c] : h[c]; }
 };
@@ -202,9 +221,9 @@ __device__ __forceinline__ auto base0_b(const Ring& ring, int k0) {
 
 // d (+)= A x B over K steps c < KS, issued by this warp group as one wgmma batch and waited for; `under` runs between the
 // commit and the wait.  Every batch of the kernel goes through here, so every accumulator gets its products in the same
-// order: pass hi*hi, lo*hi, hi*lo, the K steps inside each pass.  a(c, lo) (TileA or RegA) and bd(c, lo): the A operand
-// and the B descriptor of K step c, hi or lo part.  ACC: onto what d holds, else from 0.
-template <int N, int KS, bool ACC = false, class A, class B, class U>
+// order: pass hi*hi, lo*hi, hi*lo (the first NP of them), the K steps inside each pass.  a(c, lo) (TileA or RegA) and
+// bd(c, lo): the A operand and the B descriptor of K step c, hi or lo part.  ACC: onto what d holds, else from 0.
+template <int NP, int N, int KS, bool ACC = false, class A, class B, class U>
 __device__ __forceinline__ void mma_batch(float (&d)[N / 2], const A& a, const B& bd, U&& under) {
   if (!ACC) {
 #pragma unroll
@@ -214,7 +233,7 @@ __device__ __forceinline__ void mma_batch(float (&d)[N / 2], const A& a, const B
   a.template pin<KS>();
   tc::wgmma_fence();
 #pragma unroll
-  for (int ps = 0; ps < 3; ++ps) {
+  for (int ps = 0; ps < NP; ++ps) {
 #pragma unroll
     for (int c = 0; c < KS; ++c) wgmma<N>(d, a(c, ps == 1), bd(c, ps == 2));
   }
@@ -242,7 +261,7 @@ __device__ __forceinline__ void frag_cols(float x0, float x1, int lane, float& c
 }
 // An N = 32 fragment x (after its epilogue) -> the A fragments of the next layer's 4 K steps, split into hi / lo
 // (ah[j], al[j], j < 4)
-template <int KA>
+template <int NP, int KA>
 __device__ __forceinline__ void frag_to_a(const float (&x)[16], int lane, uint32_t (&ah)[KA][4], uint32_t (&al)[KA][4]) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -250,8 +269,8 @@ __device__ __forceinline__ void frag_to_a(const float (&x)[16], int lane, uint32
     for (int r = 0; r < 2; ++r) {
       float c0, c4;
       frag_cols(x[4 * j + 2 * r], x[4 * j + 2 * r + 1], lane, c0, c4);
-      tc::split_tf32(c0, ah[j][r], al[j][r]);                          // column 8j + q of row fr + 8r
-      tc::split_tf32(c4, ah[j][2 + r], al[j][2 + r]);                  // column 8j + q + 4
+      split<NP>(c0, ah[j][r], al[j][r]);                               // column 8j + q of row fr + 8r
+      split<NP>(c4, ah[j][2 + r], al[j][2 + r]);                       // column 8j + q + 4
     }
   }
 }
@@ -289,11 +308,12 @@ __device__ __forceinline__ void row_dot8(const float (&z)[4], const float* __res
 // issues, without leaving its registers and without meeting the other warp group: L0 reads A[0:32] from the tile (both
 // warp groups wrote it before the barrier in front of the heads), its epilogue runs on the accumulator fragment, L1 takes
 // A from registers, and the outputs go to xch slots XCH_HEAD + 2 hd + {0, 1}.  Releases the head's ring stage on its own.
+template <int NP>
 __device__ __forceinline__ void run_head(const Blk& b, Ring& ring, const float* __restrict__ hw, float* __restrict__ xo, int fr) {
   const int lane = b.row & 31, q = lane & 3;
   const uint32_t w = ring.wait(0).addr;
   float d[16];
-  mma_batch<32, 4>(d, tile_a(b, 0, 64), tile_b(w, tcl::HEAD_L0), [] {});
+  mma_batch<NP, 32, 4>(d, tile_a(b, 0, 64), tile_b(w, tcl::HEAD_L0), [] {});
   // bias + ELU, then into L1's A layout
   uint32_t ah[4][4], al[4][4];
 #pragma unroll
@@ -305,9 +325,9 @@ __device__ __forceinline__ void run_head(const Blk& b, Ring& ring, const float* 
       d[4 * j + 2 * r + 1] = elu(d[4 * j + 2 * r + 1] + bb.y);
     }
   }
-  frag_to_a(d, lane, ah, al);
+  frag_to_a<NP>(d, lane, ah, al);
   float e[16];
-  mma_batch<32, 4>(e, RegA<4>{ah, al}, tile_b(w, tcl::HEAD_L1), [] {});
+  mma_batch<NP, 32, 4>(e, RegA<4, NP>{ah, al}, tile_b(w, tcl::HEAD_L1), [] {});
   ring.release(0);
   ring.advance(1);
   // (o0, o1) of rows fr, fr + 8: this thread's 8 columns, then the quad's sum; lane q stores output q & 1 of row fr + 8 (q >> 1)
@@ -343,13 +363,14 @@ __device__ __forceinline__ void run_head(const Blk& b, Ring& ring, const float* 
 // Ring stages (each warp group waits and releases on its own): base_fc.2 (tcl::B1_L) | vis_fc.0 + vis_fc.2 (tcl::VIS0_L,
 // VIS2_L) | vis_fc2.0 + rgb_fc.0 (tcl::V20_L, RGB0_L).
 // tk: where the phase stamps after base_fc.2, vis_fc.0, vis_fc.2 and vis_fc2.0 go (nullptr: none).
+template <int NP>
 __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float* __restrict__ sw, float* __restrict__ xch, int fr, long long* tk) {
   const int lane = b.row & 31, q = lane & 3;
   // base_fc.2: K = 64 from the tile; the row scalars load under its MMAs
   uint32_t w = ring.wait(0).addr;
   float d[16];
   float w1[2], mr[2], t0[2], t1[2];                 // t0, t1: rgb_fc.0's K tail, columns 32 + q and 36 + q (t0 of lane 0 is vis2)
-  mma_batch<32, 8>(d, tile_a(b, 0, 64), tile_b(w, tcl::B1_L), [&] {
+  mma_batch<NP, 32, 8>(d, tile_a(b, 0, 64), tile_b(w, tcl::B1_L), [&] {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const float* __restrict__ x = xch + XCH_FRONT * 128 + fr + 8 * r;
@@ -371,11 +392,11 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
     }
   }
   uint32_t ah[4][4], al[4][4];
-  frag_to_a(xr, lane, ah, al);
+  frag_to_a<NP>(xr, lane, ah, al);
   if (tk) tk[0] = clock64();
   // vis_fc.0 (row scale w1 in the epilogue)
   w = ring.wait(1).addr;
-  mma_batch<32, 4>(d, RegA<4>{ah, al}, tile_b(w, tcl::VIS0_L), [] {});
+  mma_batch<NP, 32, 4>(d, RegA<4, NP>{ah, al}, tile_b(w, tcl::VIS0_L), [] {});
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const float2 bb = *reinterpret_cast<const float2*>(sw + SW_V0B + 8 * j + 2 * q);
@@ -385,11 +406,11 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
       d[4 * j + 2 * r + 1] = elu(fmaf(w1[r], d[4 * j + 2 * r + 1], bb.y));
     }
   }
-  frag_to_a(d, lane, ah, al);
+  frag_to_a<NP>(d, lane, ah, al);
   if (tk) tk[1] = clock64();
   // vis_fc.2, then vis_fc.1 (the vis_fc.0 outputs' dot product; under the MMAs, with their A registers pinned, it spills)
   float e[16];
-  mma_batch<32, 4>(e, RegA<4>{ah, al}, tile_b(w, tcl::VIS2_L), [] {});
+  mma_batch<NP, 32, 4>(e, RegA<4, NP>{ah, al}, tile_b(w, tcl::VIS2_L), [] {});
   ring.release(1);
   float visa[2];
   {
@@ -409,11 +430,11 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
     }
   }
   uint32_t a2h[5][4], a2l[5][4];
-  frag_to_a(xr, lane, a2h, a2l);
+  frag_to_a<NP>(xr, lane, a2h, a2l);
   if (tk) tk[2] = clock64();
   // vis_fc2.0; x2 goes to the tile under its MMAs
   w = ring.wait(2).addr;
-  mma_batch<32, 4>(d, RegA<5>{a2h, a2l}, tile_b(w, tcl::V20_L), [&] { tc::acc_store_half<32>(b.act, 96, b.row, b.wg, xr); });
+  mma_batch<NP, 32, 4>(d, RegA<5, NP>{a2h, a2l}, tile_b(w, tcl::V20_L), [&] { tc::acc_store_half<32>(b.act, 96, b.row, b.wg, xr); });
   float vis2[2];
   {
 #pragma unroll
@@ -434,11 +455,11 @@ __device__ __forceinline__ void run_chain(const Blk& b, Ring& ring, const float*
   // rgb_fc.0: K = 32 (x2) + the tail (vis2, dd0, dd1, dd2 | dd3, 0, 0, 0), N = 16
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    tc::split_tf32(q == 0 ? vis2[r] : t0[r], a2h[4][r], a2l[4][r]);
-    tc::split_tf32(t1[r], a2h[4][2 + r], a2l[4][2 + r]);
+    split<NP>(q == 0 ? vis2[r] : t0[r], a2h[4][r], a2l[4][r]);
+    split<NP>(t1[r], a2h[4][2 + r], a2l[4][2 + r]);
   }
   float g[8];
-  mma_batch<16, 5>(g, RegA<5>{a2h, a2l}, tile_b(w, tcl::RGB0_L), [&] {
+  mma_batch<NP, 16, 5>(g, RegA<5, NP>{a2h, a2l}, tile_b(w, tcl::RGB0_L), [&] {
     if (q < 2) xch[XCH_L2 * 128 + fr + 8 * q] = q ? vis2[1] : vis2[0];
   });
   ring.release(2);
@@ -465,16 +486,16 @@ __device__ __forceinline__ void ld_own(const Blk& b, int col, float* v) {
     v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
   }
 }
-// the same columns of a row of activations -> hi parts from `hi`, lo parts from `lo`
-template <int Q>
+// the same columns of a row of activations -> hi parts from `hi`, lo parts from `lo` (NP = 3 only)
+template <int NP, int Q>
 __device__ __forceinline__ void st_own(const Blk& b, int hi, int lo, const float* v) {
 #pragma unroll
   for (int q = 0; q < Q; ++q) {
     uint32_t h[4], l[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) tc::split_tf32(v[4 * q + j], h[j], l[j]);
+    for (int j = 0; j < 4; ++j) split<NP>(v[4 * q + j], h[j], l[j]);
     *reinterpret_cast<uint4*>(b.act + own_index(b, hi + 8 * q)) = make_uint4(h[0], h[1], h[2], h[3]);
-    *reinterpret_cast<uint4*>(b.act + own_index(b, lo + 8 * q)) = make_uint4(l[0], l[1], l[2], l[3]);
+    if constexpr (NP == 3) *reinterpret_cast<uint4*>(b.act + own_index(b, lo + 8 * q)) = make_uint4(l[0], l[1], l[2], l[3]);
   }
 }
 // entries 8q + 4 wg + [0,4) of a weight or bias vector (shared memory, 16-byte aligned)
@@ -500,8 +521,9 @@ __device__ __forceinline__ void ld_row(const Blk& b, int col, float* v) {
   }
 }
 
-template <int G, bool DEBUG>
-__global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
+// The kernel body, NP passes per tensor-core product (point_kernel_pm3: 3, point_kernel_tf32: 1)
+template <int G, bool DEBUG, int NP>
+__device__ __forceinline__ void point_body(const KParams& kp) {
   extern __shared__ __align__(1024) float smem[];
   constexpr bool P2 = (G & (G - 1)) == 0;      // power-of-two lane groups reduce with butterflies, the others through shared memory
   constexpr int PPW = 32 / G;                   // points per warp (G = 10: 3, two lanes idle)
@@ -735,7 +757,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         const float4 t4 = *reinterpret_cast<const float4*>(stg + lane * STG_ROW + 4 * q);
         x[4 * q] = t4.x; x[4 * q + 1] = t4.y; x[4 * q + 2] = t4.z; x[4 * q + 3] = t4.w;
       }
-      st_own<4>(b, 0, 64, x);
+      st_own<NP, 4>(b, 0, 64, x);
       if (DEBUG && kp.dbg != nullptr && row_ok) {
         float* __restrict__ o = kp.dbg + (size_t(v) * N + n) * 76;
         for (int k = 0; k < 16; ++k) o[12 + 8 * (k >> 2) + 4 * wg + (k & 3)] = x[k];
@@ -764,7 +786,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     tc::fence_proxy_async_smem();
     tc::named_sync(BAR_LAYER, NCOMP);
 #pragma unroll 1
-    for (int hd = 0; hd < n_heads; ++hd) run_head(b, ring, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
+    for (int hd = 0; hd < n_heads; ++hd) run_head<NP>(b, ring, sw + SW_HEAD + hd * SW_HEAD_STRIDE, xch + (XCH_HEAD + 2 * hd) * 128, fr);
     PM_TICK(4)
 
     // ---------------- the front, hit/vis through base_fc.0: each warp group for its own 64 rows, in its accumulator fragment ----------------
@@ -830,12 +852,14 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           uint32_t h, l;
-          tc::split_tf32(q < 2 ? (r ? other : hv01) : 0.f, h, l);
+          split<NP>(q < 2 ? (r ? other : hv01) : 0.f, h, l);
           const int rr = fr_f + 8 * r;
           at[tc::act_index(rr, 32 + q)] = h;
-          at[tc::act_index(rr, 96 + q)] = l;
           at[tc::act_index(rr, 36 + q)] = 0u;
-          at[tc::act_index(rr, 100 + q)] = 0u;
+          if constexpr (NP == 3) {
+            at[tc::act_index(rr, 96 + q)] = l;
+            at[tc::act_index(rr, 100 + q)] = 0u;
+          }
         }
       }
       tc::fence_proxy_async_smem();
@@ -844,7 +868,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       uint32_t ah[4][4], al[4][4];
       {
         float d[16];
-        mma_batch<32, 5>(d, tile_a(b, 0, 64), tile_b(ring.wait(0).addr, tcl::PE0_L), [] {});
+        mma_batch<NP, 32, 5>(d, tile_a(b, 0, 64), tile_b(ring.wait(0).addr, tcl::PE0_L), [] {});
         ring.release(0);
         ring.advance(1);
 #pragma unroll
@@ -856,14 +880,14 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
             d[4 * j + 2 * r + 1] = fmaxf(d[4 * j + 2 * r + 1] + bb.y, 0.f);
           }
         }
-        frag_to_a(d, lane_f, ah, al);
+        frag_to_a<NP>(d, lane_f, ah, al);
       }
       PM_TICK(5)
       // prob_embed.2 with neuray_fc.0 behind it (N = 48): neuray_feat = columns [0,32) + bias, the gate from columns [32,40)
       float gate[2];
       {
         float d[24];
-        mma_batch<48, 4>(d, RegA<4>{ah, al}, tile_b(ring.wait(0).addr, tcl::PE1_L), [] {});
+        mma_batch<NP, 48, 4>(d, RegA<4, NP>{ah, al}, tile_b(ring.wait(0).addr, tcl::PE1_L), [] {});
         ring.release(0);
         ring.advance(1);
 #pragma unroll
@@ -887,7 +911,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         float nf[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) nf[j] = d[j];
-        frag_to_a(nf, lane_f, ah, al);
+        frag_to_a<NP>(nf, lane_f, ah, al);
       }
       // base_fc.0, K round A: the neuray_feat inputs (its K steps 5..8).  Waits for all three of its stages, which round B
       // reads too.  Under its MMAs: the gate goes to the row owners' slot, and ray_dir_fc.0 (K 4, N 16) runs on the CUDA
@@ -897,7 +921,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       ring.wait(2);
       float acc[32];
       uint32_t rh[2][4], rl[2][4];
-      mma_batch<64, 4>(acc, RegA<4>{ah, al}, base0_b(ring, 5), [&] {
+      mma_batch<NP, 64, 4>(acc, RegA<4, NP>{ah, al}, base0_b(ring, 5), [&] {
         if (q < 2) xch[XCH_GATE * 128 + fr_f + 8 * q] = q ? gate[1] : gate[0];
         const float* __restrict__ w0 = sw + SW_RD0W;
 #pragma unroll
@@ -910,14 +934,14 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
             for (int h = 0; h < 2; ++h) {
               const int u = 8 * s + 4 * h + q;
               const float x = elu(fmaf(w0[48 + u], d3, fmaf(w0[32 + u], d2, fmaf(w0[16 + u], d1, fmaf(w0[u], d0, sw[SW_RD0B + u])))));
-              tc::split_tf32(x, rh[s][2 * h + r], rl[s][2 * h + r]);
+              split<NP>(x, rh[s][2 * h + r], rl[s][2 * h + r]);
             }
           }
         }
       });
       // ray_dir_fc.2: K = 16, N = 48 (35 used)
       float e[24];
-      mma_batch<48, 2>(e, RegA<2>{rh, rl}, tile_b(tc::smem_u32(smem + OFF_RD1), tcl::RD1_L), [] {});
+      mma_batch<NP, 48, 2>(e, RegA<2, NP>{rh, rl}, tile_b(tc::smem_u32(smem + OFF_RD1), tcl::RD1_L), [] {});
       // rgb_feat (35) + the constant 1 (column 35: base_fc.0's bias) + zero padding, in round B's A fragments.  Column c < 35
       // is elu(ray_dir_fc.2 + bias) + rgbin[c] (c < 3) or img_feats channel c - 3, which warp group ((c - 3) >> 2) & 1
       // gathered into its buffer column 4 ((c - 3) >> 3) + ((c - 3) & 3), row rr at lane rr & 31 of its warp rr >> 5.
@@ -948,13 +972,13 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
                 if (s < 4) rfo[(2 * s + h) * 256 + 32 * r] = f;
                 else xch[(XCH_RF + q) * 128 + fr_f + 8 * r] = f;
               }
-              tc::split_tf32(f, bh[s][2 * h + r], bl[s][2 * h + r]);
+              split<NP>(f, bh[s][2 * h + r], bl[s][2 * h + r]);
             }
           }
         }
       }
       // base_fc.0, K round B: rgb_feat (its K steps 0..4), onto round A's accumulators
-      mma_batch<64, 5, true>(acc, RegA<5>{bh, bl}, base0_b(ring, 0), [] {});
+      mma_batch<NP, 64, 5, true>(acc, RegA<5, NP>{bh, bl}, base0_b(ring, 0), [] {});
 #pragma unroll
       for (int s = 0; s < 3; ++s) ring.release(s);
       ring.advance(3);
@@ -991,7 +1015,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
     {
       const float c1 = 2.f - gsum(w1), c0 = 2.f - gsum(w0);
       float* const op = b.act;
-      PtAcc<PB> acc = {};
+      PtAcc<PB, NP> acc = {};
       auto round = [&](auto rc) {
         constexpr int R = decltype(rc)::value;
         float in[16], st[16];
@@ -1010,7 +1034,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         put_point(op, 32 * R, st);
         tc::named_sync(BAR_LAYER, NCOMP);
         if (R > 0) ring.release(R - 1);
-        point_mma<PB, 4>(acc, op, 32 * R, ring.wait(R).p, tcl::HST_STAGE, warp, lane);
+        point_mma<PB, 4, NP>(acc, op, 32 * R, ring.wait(R).p, tcl::HST_STAGE, warp, lane);
       };
       round(std::integral_constant<int, 0>{}); round(std::integral_constant<int, 1>{}); round(std::integral_constant<int, 2>{});
       round(std::integral_constant<int, 3>{}); round(std::integral_constant<int, 4>{});
@@ -1030,7 +1054,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       add_bias_own<4>(b, x, smem + OFF_PT + pq * PT_ROW + c0);
 #pragma unroll
       for (int j = 0; j < 16; ++j) x[j] = elu(x[j]);
-      st_own<4>(b, c0, 64 + c0, x);                                                // lo half 1 lands on accumulator columns already consumed
+      st_own<NP, 4>(b, c0, 64 + c0, x);                                                // lo half 1 lands on accumulator columns already consumed
     }
     if (wg == 0) xch[XCH_W1 * 128 + row] = w1;                                     // w1 of the chain's fragment rows
     PM_TICK(8)
@@ -1042,7 +1066,7 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
       if constexpr (DEBUG) {
         if (kp.timing != nullptr && blockIdx.x == 0 && row == 0 && it < 64) tk = kp.timing + (it * 2 + wg) * 32 + 9;
       }
-      run_chain(b, ring, sw, xch, fr, tk);
+      run_chain<NP>(b, ring, sw, xch, fr, tk);
     }
     tc::named_sync(BAR_LAYER, NCOMP);                                              // x2, rgb_fc.0 and vis2 -> the row owners
     float xr[16];
@@ -1081,12 +1105,12 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
         *reinterpret_cast<float4*>(op + pl * OP_ROW + 68) = make_float4(0.f, 0.f, 0.f, 0.f);
       }
       tc::named_sync(BAR_LAYER, NCOMP);
-      PtAcc<PB> acc = {};
+      PtAcc<PB, NP> acc = {};
 #pragma unroll
       for (int s = 0; s < 3; ++s) {
         const float* w = ring.wait(s).p;
-        if (s < 2) point_mma<PB, 4>(acc, op, 32 * s, w, tcl::G0_L, warp, lane);
-        else point_mma<PB, 1>(acc, op, 64, w, tcl::G0_L, warp, lane);
+        if (s < 2) point_mma<PB, 4, NP>(acc, op, 32 * s, w, tcl::G0_L, warp, lane);
+        else point_mma<PB, 1, NP>(acc, op, 64, w, tcl::G0_L, warp, lane);
       }
       point_store(acc, smem + OFF_PT, warp, lane);
       tc::named_sync(BAR_LAYER, NCOMP);                                            // per-point result visible; the stages read
@@ -1166,5 +1190,12 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) {
   }
 #undef PM_TICK
 }
+
+template <int G, bool DEBUG>
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) { point_body<G, DEBUG, 3>(kp); }
+// TF32 mode (release form only): one tensor-core pass per product, operands rounded to nearest, B from a pack with
+// rna(W) in the hi slots (nr_pack_weights_tf32)
+template <int G>
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_tf32(const KParams kp) { point_body<G, false, 1>(kp); }
 
 }  // namespace pm3

@@ -12,6 +12,7 @@
 //   * fp32 accuracy comes from the 3xTF32 split: x = hi + lo with hi = x & 0xffffe000 (exactly representable in
 //     tf32, so it does not matter whether the tensor core truncates or rounds), lo = x - hi (exact);
 //     D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo
+//   * the point kernel's TF32 mode issues only the first of these passes, on operands rounded to nearest (tf32_rna)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -243,6 +244,13 @@ __device__ __forceinline__ void acc_store(float* act, int dcol, int t, const flo
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xffffe000u;
   lo = __float_as_uint(x - __uint_as_float(hi));
+}
+// one-pass TF32 operand: x rounded to the nearest tf32 value (ties away from zero; the low 13 bits come out zero).  A
+// truncated operand would bias every product of a K-long sum the same way.
+__device__ __forceinline__ uint32_t tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
+  return r;
 }
 
 // ---- mma.sync (one warp) ----

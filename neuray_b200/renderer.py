@@ -23,7 +23,7 @@ import torch.nn as nn
 
 from . import _lib, encoders, init_nets, modules
 from .render_ops import fine_sample_u, interpolate_feats, sample_depth
-from .weights import camera_blocks, pack_pass, point_index_map, posenc_table
+from .weights import camera_blocks, pack_pass, pack_pass_tf32, point_index_map, posenc_table
 
 PACK_KEY = "_nr_frame_pack"        # ref_imgs_info: the FramePack of the frame being rendered (lives for one render() call)
 CAM_KEY = "_nr_que_cam"            # que_imgs_info: que_cam block of the frame being rendered (same lifetime)
@@ -41,6 +41,26 @@ base_cfg = {
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
+
+
+# Arithmetic of the point kernel's tensor-core layers in render passes that record no gradient.
+# "fp32": 3xTF32, fp32 accuracy (the default).  "tf32": one TF32 pass per product on operands rounded to nearest, what
+# torch 1.7 to 1.11 ran nn.Linear in on Ampere and later GPUs by default (the reference pins torch 1.7.1); about 1e-3
+# relative per layer.  The ray kernel and the encoders (encoders.set_precision) do not depend on it.
+PRECISION = "fp32"
+
+
+def set_precision(mode):
+    """Selects the render passes' point-kernel arithmetic: "fp32" (3xTF32) or "tf32" (one TF32 pass per product).
+
+    A pass that records a gradient (autograd on, and a parameter or the feature maps require grad) always runs in fp32:
+    nr_render_pass_bwd recomputes the forward in fp32, so a TF32 forward would return values of a different function
+    than the one its gradients belong to.  Under torch.no_grad() (inference, the validation loop of run_training.py)
+    "tf32" applies to every pass, whichever entry point reaches it."""
+    global PRECISION
+    if mode not in ("fp32", "tf32"):
+        raise ValueError(f"render precision {mode!r}: 'fp32' or 'tf32'")
+    PRECISION = mode
 
 
 # Grow-only device workspaces, reused across passes, chunks and frames.  The C-ABI never allocates (the caller owns
@@ -151,10 +171,11 @@ def _pass_modules(owner, is_fine):
         (owner.dist_decoder, owner.agg_net, "dist_decoder", "agg_net")
 
 
-def pass_weights(owner, is_fine, dn, device):
+def pass_weights(owner, is_fine, dn, device, tf32=False):
     """Packed weights of one pass (nr_pack_weights), cached on the owner and re-packed when any parameter changed
     (optimizer steps bump tensor._version).  Every re-pack gets fresh buffers: an autograd graph recorded before the
-    parameter update keeps reading the buffers it was recorded with."""
+    parameter update keeps reading the buffers it was recorded with.  tf32: w_tc is the TF32 mode's pack
+    (nr_pack_weights_tf32), made on first use after each re-pack and cached next to the other one."""
     dec, agg, dec_name, agg_name = _pass_modules(owner, is_fine)
     params = {f"{dec_name}.{k}": v for k, v in dec.named_parameters()}
     params.update({f"{agg_name}.{k}": v for k, v in agg.named_parameters()})
@@ -166,7 +187,7 @@ def pass_weights(owner, is_fine, dn, device):
         if first.device != torch.device(device):
             raise _lib.NeurayB200Error(f"parameters live on {first.device} but the rays are on {device}")
         wp, wr, wt = pack_pass(params, dec_name, agg_name)
-        hit = (stamp, wp, wr, hit[3] if hit is not None else {}, wt)
+        hit = (stamp, wp, wr, hit[3] if hit is not None else {}, wt, {})
         cache[is_fine] = hit
     pe = hit[3].get(dn)
     if pe is None:
@@ -177,7 +198,12 @@ def pass_weights(owner, is_fine, dn, device):
                 f"{agg_name}: pos_encoding was built for sample_num={n_samples} but the pass has {dn} samples per ray")
         pe = posenc_table(dn).to(device).contiguous()
         hit[3][dn] = pe
-    return hit[1], hit[2], pe, hit[4]
+    if not tf32:
+        return hit[1], hit[2], pe, hit[4]
+    wt = hit[5].get("tf32")
+    if wt is None:
+        wt = hit[5]["tf32"] = pack_pass_tf32(params, dec_name, agg_name)
+    return hit[1], hit[2], pe, wt
 
 
 def pass_index_map(owner, is_fine, dev):
@@ -233,15 +259,16 @@ def _direct_render(owner, out, rn, dn, dev):
     return res
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit):
-    """Enqueues the two kernels of one pass; returns the raw output dict (ray_mask as uint8)."""
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit, tf32=False):
+    """Enqueues the two kernels of one pass; returns the raw output dict (ray_mask as uint8).  tf32: the point kernel in
+    TF32 mode (set_precision)."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
     pack = frame_pack(ref_imgs_info)
     _, rn, dn = que_depth.shape
     dec, agg, _, _ = _pass_modules(owner, is_fine)
-    w_point, w_ray, pos_enc, w_tc = pass_weights(owner, is_fine, dn, dev)
+    w_point, w_ray, pos_enc, w_tc = pass_weights(owner, is_fine, dn, dev, tf32)
     cam = que_imgs_info.get(CAM_KEY)
     if cam is None:
         cam, _ = camera_blocks(que_imgs_info, None)
@@ -284,11 +311,16 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
             # bench.py: time the dominant kernel alone, with CUDA events on the launching stream
             e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
             e0.record()
-            _lib.check(_lib.lib().nr_point_kernel(C.byref(p), stream), "nr_point_kernel")
+            if tf32:
+                _lib.check(_lib.lib().nr_point_kernel_tf32(C.byref(p), stream), "nr_point_kernel_tf32")
+            else:
+                _lib.check(_lib.lib().nr_point_kernel(C.byref(p), stream), "nr_point_kernel")
             e1.record()
             _lib.check(_lib.lib().nr_ray_kernel(C.byref(p), stream), "nr_ray_kernel")
             e2.record()
             _lib.PROFILE.append((e0, e1, rn * dn, e2))
+        elif tf32:
+            _lib.check(_lib.lib().nr_render_pass_fwd_tf32(C.byref(p), stream), "nr_render_pass_fwd_tf32")
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
     _lib.count_launches(2)
@@ -304,7 +336,8 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
-    outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels)."""
+    outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
+    pass runs in fp32 whatever set_precision chose: the backward recomputes it in fp32.  Otherwise PRECISION applies."""
     coords = que_imgs_info["coords"]
     if coords.shape[0] != 1:
         raise _lib.NeurayB200Error("one query view per call (qn == 1), like every call site of the reference")
@@ -317,9 +350,10 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     named = [(f"{dec_name}.{k}", v) for k, v in dec.named_parameters()] + [(f"{agg_name}.{k}", v) for k, v in agg.named_parameters()]
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for _, v in named))
     dr = {} if owner.cfg["use_dr_prediction"] else None
+    tf32 = PRECISION == "tf32" and not needs_grad
 
     def launch():
-        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit)
+        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit, tf32)
         if dr is not None:
             dr.update(_direct_render(owner, out, rn, dn, coords.device))
         return out

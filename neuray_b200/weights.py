@@ -80,6 +80,18 @@ def pack_pass(params, dec, agg, out=None):
     return out
 
 
+def pack_pass_tf32(params, dec, agg):
+    """w_tc of one pass for the point kernel's TF32 mode (nr_pack_weights_tf32: the same layout, rna(W) in the hi slots)."""
+    any_t = params[f"{dec}.mean_decoder.0.weight"]
+    out = torch.empty(_lib.tc_layout().total, dtype=torch.float32, device=any_t.device)
+    w, keep = pass_weight_struct(params, dec, agg)
+    with _lib.on_device(any_t):
+        _lib.check(_lib.lib().nr_pack_weights_tf32(C.byref(w), _lib.ptr(out), _lib.stream_of(any_t)), "nr_pack_weights_tf32")
+    _lib.count_launches(1)
+    del keep
+    return out
+
+
 def point_index_map(params, dec, agg):
     """For the packed-layout gradient of nr_self_hit_prob: position in w_point -> 1 + flat index into the concatenated
     parameters (0 = padding), derived by packing parameters whose elements are their own index (exact in fp32 < 2^24)."""
