@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 10
+#define NR_ABI_VERSION 11
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -183,6 +183,19 @@ typedef struct NrDrParams {
   float* hit_prob_dr;        /* [rn,dn] */
 } NrDrParams;
 int nr_direct_render(const NrPassParams* p, const NrDrParams* d, void* stream);
+
+/* Per-view visibility of each rendered pixel (cfg render_visibility): visibility[r, v] = Σ_d hit_prob[r, d] · vis_v[r, d],
+ * where vis_v is the reference's masked prj_dict['vis'] of the same pass (renderer.py:79-82: compute_prob's visibility
+ * of the active pass' dist decoder, times the projection mask), recomputed per (point, view) in fp32, and hit_prob the
+ * pass' compositing weight (hit_prob_nr).  Views in view_params order; unnormalised, like render_depth.  Enqueue it after
+ * nr_render_pass_fwd (or _tf32) of the same NrPassParams: it reads the pass' inputs and its hit_prob.  Each ray's sum
+ * runs in an order fixed by dn alone, so a ray's result does not depend on the chunk or launch that renders it.
+ * One kernel, no host synchronisation, no workspace. */
+typedef struct NrVisParams {
+  const float* hit_prob;     /* [rn,dn]: the pass' hit_prob output */
+  float* visibility;         /* [rn,rfn] */
+} NrVisParams;
+int nr_view_visibility(const NrPassParams* p, const NrVisParams* v, void* stream);
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);

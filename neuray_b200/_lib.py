@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -48,6 +48,10 @@ class NrDrParams(C.Structure):
                 ("point_colors", C.c_void_p), ("pixel_colors_dr", C.c_void_p), ("hit_prob_dr", C.c_void_p)]
 
 
+class NrVisParams(C.Structure):
+    _fields_ = [("hit_prob", C.c_void_p), ("visibility", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -78,6 +82,7 @@ SIGNATURES = {
     "nr_render_pass_fwd": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_render_pass_fwd_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_direct_render": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrDrParams), _vp]),
+    "nr_view_visibility": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrVisParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),

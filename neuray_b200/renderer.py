@@ -38,6 +38,8 @@ base_cfg = {
     "use_dr_prediction": False, "use_nr_color_for_dr": False, "use_self_hit_prob": False,
     "use_ray_mask": True, "ray_mask_view_num": 2, "ray_mask_point_num": 8,
     "render_depth": False,
+    # each pass' visibility_nr [1,rn,rfn]: every pixel's visibility from each working view (nr_view_visibility)
+    "render_visibility": False,
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
@@ -259,6 +261,21 @@ def _direct_render(owner, out, rn, dn, dev):
     return res
 
 
+def _view_visibility(out, rn, rfn, dev):
+    """render_visibility: nr_view_visibility enqueued right behind the pass whose raw outputs `out` holds, on its
+    hit_prob.  Returns visibility [1,rn,rfn]: Σ_d hit_prob · the masked prj_dict['vis'] of each view (renderer.py:79-82)."""
+    vis = torch.empty(1, rn, rfn, dtype=torch.float32, device=dev)
+    if out["_bwd"] is None:          # rn == 0: nothing was launched
+        return vis
+    p, _keep, _, stream = out["_bwd"]
+    q = _lib.NrVisParams()
+    q.hit_prob, q.visibility = _lib.ptr(out["hit_prob"]), _lib.ptr(vis)
+    with _lib.on_device(vis):
+        _lib.check(_lib.lib().nr_view_visibility(C.byref(p), C.byref(q), stream), "nr_view_visibility")
+    _lib.count_launches(1)
+    return vis
+
+
 def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit, tf32=False):
     """Enqueues the two kernels of one pass; returns the raw output dict (ray_mask as uint8).  tf32: the point kernel in
     TF32 mode (set_precision)."""
@@ -332,8 +349,9 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
 def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None, want_hit=True):
     """One fused pass.  que_depth [1,rn,dn].  `fine`: None or dict(dn=, use_all=, u=, u_stride=) to also emit the
     next pass' depths.  Returns dict with pixel_colors [1,rn,3], hit_prob [1,rn,dn], render_depth [1,rn],
-    ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M] and, with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
-    hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises).
+    ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M], with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
+    hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises) and, with cfg
+    render_visibility, visibility [1,rn,rfn] (no gradient: requires_grad is False).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
@@ -350,12 +368,15 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     named = [(f"{dec_name}.{k}", v) for k, v in dec.named_parameters()] + [(f"{agg_name}.{k}", v) for k, v in agg.named_parameters()]
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for _, v in named))
     dr = {} if owner.cfg["use_dr_prediction"] else None
+    vis = {} if owner.cfg.get("render_visibility", False) else None
     tf32 = PRECISION == "tf32" and not needs_grad
 
     def launch():
-        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit, tf32)
+        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit or vis is not None, tf32)
         if dr is not None:
             dr.update(_direct_render(owner, out, rn, dn, coords.device))
+        if vis is not None:
+            vis["visibility"] = _view_visibility(out, rn, rf.shape[0], coords.device)
         return out
     if not needs_grad:
         out = launch()
@@ -372,6 +393,8 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
             dr = dict(zip(("pixel_colors_dr", "hit_prob_dr"), DirectRenderFn.apply(dr, rf, imf, *[v for _, v in named])))
     if dr is not None:
         out.update(dr)
+    if vis is not None:
+        out.update(vis)
     out["ray_mask"] = out.pop("ray_mask_u8").bool()
     return out
 
@@ -387,6 +410,8 @@ def _finish_outputs(owner, res, que_depth, que_imgs_info):
         outputs["ray_mask"] = res["ray_mask"]
     if cfg["render_depth"]:
         outputs["render_depth"] = res["render_depth"]
+    if cfg.get("render_visibility", False):
+        outputs["visibility_nr"] = res["visibility"]
     return outputs
 
 
