@@ -8,19 +8,11 @@ import ctypes as C
 import torch
 
 from . import _lib
+from .weights import HEADS
 
-HEADS = ("mean_decoder", "var_decoder", "aw_decoder", "vis_decoder")
-_WS = {}
-
-
-def _ws(key, numel, dev):
-    buf = _WS.get((key, str(dev)))
-    if buf is None or buf.numel() < numel:
-        _WS.pop((key, str(dev)), None)
-        buf = torch.empty(numel, dtype=torch.float32, device=dev)
-        _WS[(key, str(dev))] = buf
-    return buf[:numel]
-
+# the tapes live in the package's one workspace pool; under this name too, as the tests that pre-fill them with NaN
+# (a kernel reading an unwritten slot then yields a NaN gradient) have always addressed them
+_WS = _lib.WORKSPACES
 
 TILE = 128
 
@@ -160,7 +152,7 @@ def render_pass_backward(p, names, dec, agg, g_pix, g_hit, g_depth, want_feat_gr
     dev = (g_pix if g_pix is not None else g_hit if g_hit is not None else g_depth).device
     n_points = p.rn * p.dn
     shapes = tape_shapes(p.rfn, n_points)
-    bufs = {k: _ws(k, sh[0] * sh[1] * sh[2], dev).view(sh) for k, sh in shapes.items()}
+    bufs = {k: _lib.workspace(k, sh[0] * sh[1] * sh[2], dev).view(sh) for k, sh in shapes.items()}
     d_feat = torch.zeros(feat_shape, dtype=torch.float32, device=dev) if want_feat_grads else None
     b = _lib.NrBwdParams()
     keep = [t.contiguous().float() if t is not None else None for t in (g_pix, g_hit, g_depth)]
@@ -191,14 +183,13 @@ def unpack_point_grads(index_map, d_w_point):
 
 
 class RenderPassFn(torch.autograd.Function):
-    """forward = the fused CUDA pass (values), backward = nr_render_pass_bwd + nr_tape_gemms."""
+    """forward = the outputs of the fused CUDA pass that `launch` (renderer.PassLaunch, None for an empty chunk)
+    describes, backward = nr_render_pass_bwd + nr_tape_gemms on that launch's inputs."""
 
     @staticmethod
-    def forward(ctx, runner, meta, ray_feats, img_feats, *params):
-        with torch.no_grad():
-            res = runner()
+    def forward(ctx, launch, res, meta, ray_feats, img_feats, *params):
         ctx.meta = meta
-        ctx.bwd = res.pop("_bwd", None)
+        ctx.launch = launch
         ctx.save_for_backward(ray_feats, img_feats, *params)
         ctx.mark_non_differentiable(res["ray_mask_u8"])
         fine = res.get("fine_depth")
@@ -210,17 +201,16 @@ class RenderPassFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_pix, g_hit, g_depth, *unused):
-        meta = ctx.meta
+        meta, launch = ctx.meta, ctx.launch
         ray_feats, img_feats, *params = ctx.saved_tensors
-        if ctx.bwd is None:          # an empty chunk: nothing was launched, nothing flows back
-            return (None, None, None, None, *[None] * len(params))
-        p, _keep, feat_shape, stream = ctx.bwd
+        if launch is None:          # an empty chunk: nothing was launched, nothing flows back
+            return (None, None, None, None, None, *[None] * len(params))
         want_feat = ray_feats.requires_grad or img_feats.requires_grad
         with _lib.on_device(ray_feats):
-            grads, drf, dimf = render_pass_backward(p, meta["names"], meta["dec"], meta["agg"], g_pix, g_hit, g_depth, want_feat,
-                                                    feat_shape, stream)
+            grads, drf, dimf = render_pass_backward(launch.params, meta["names"], meta["dec"], meta["agg"], g_pix, g_hit, g_depth,
+                                                    want_feat, launch.feat_shape, launch.stream)
         gp = [grads[n] if t.requires_grad else None for n, t in zip(meta["names"], params)]
-        return (None, None, drf if ray_feats.requires_grad else None, dimf if img_feats.requires_grad else None, *gp)
+        return (None, None, None, drf if ray_feats.requires_grad else None, dimf if img_feats.requires_grad else None, *gp)
 
 
 class DirectRenderFn(torch.autograd.Function):

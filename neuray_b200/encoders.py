@@ -136,17 +136,6 @@ def set_precision(mode):
         raise ValueError(f"encoder precision {mode!r}: 'fp32' or 'tf32'")
     PRECISION = mode
 
-_WS = {}
-
-
-def _workspace(key, nbytes, dev):
-    buf = _WS.get((key, str(dev)))
-    if buf is None or buf.numel() < nbytes:
-        _WS.pop((key, str(dev)), None)
-        buf = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _WS[(key, str(dev))] = buf
-    return buf
-
 
 def _packed(module, names, which, dev):
     """Packed parameter buffer of an encoder (nr_*_encoder_pack), cached on the module, re-packed when a parameter changed."""
@@ -191,7 +180,7 @@ def image_encoder_into(module, imgs, out, out_off):
     dev = imgs.device
     packed = _packed(module, image_param_names(), "image", dev)
     nbytes = _lib.lib().nr_image_encoder_workspace(n, h, w)
-    ws = _workspace("image", nbytes, dev)
+    ws = _lib.workspace("image", nbytes, dev, torch.uint8)
     x = imgs.detach().contiguous().float()
     with _lib.on_device(imgs):
         _lib.check(_lib.lib().nr_image_encoder_fwd(_lib.ptr(packed), _lib.ptr(x), n, h, w, _lib.ptr(out), out.shape[-1], out_off, int(PRECISION == "tf32"),
@@ -208,7 +197,7 @@ def vis_encoder_inplace(module, feat):
     dev = feat.device
     packed = _packed(module, vis_param_names(), "vis", dev)
     nbytes = _lib.lib().nr_vis_encoder_workspace(n, fh, fw)
-    ws = _workspace("vis", nbytes, dev)
+    ws = _lib.workspace("vis", nbytes, dev, torch.uint8)
     with _lib.on_device(feat):
         _lib.check(_lib.lib().nr_vis_encoder_fwd(_lib.ptr(packed), _lib.ptr(feat), n, fh, fw, int(PRECISION == "tf32"), ws.data_ptr(), nbytes, _lib.stream_of(feat)),
                    "nr_vis_encoder_fwd")

@@ -73,7 +73,7 @@ def forward_into(module, ref_imgs_info, out, out_off):
     diff = init_ops.get_diff_feats(ref_imgs_info, depth)
     packed = encoders._packed(module, param_names(), "depth_init", dev)
     nbytes = _lib.lib().nr_depth_init_workspace(rfn, h, w)
-    ws = encoders._workspace("depth_init", nbytes, dev)
+    ws = _lib.workspace("depth_init", nbytes, dev, torch.uint8)
     x = imgs.detach().contiguous().float()
     with _lib.on_device(imgs):
         _lib.check(_lib.lib().nr_depth_init_fwd(_lib.ptr(packed), _lib.ptr(x), _lib.ptr(depth), _lib.ptr(diff.contiguous()), rfn, h, w, _lib.ptr(out),
@@ -239,7 +239,7 @@ def mvsnet_cost_volume(module, ref_imgs_info, src_imgs_info, is_train):
     nbytes = _lib.lib().nr_mvsnet_workspace(C.byref(a))
     if nbytes <= 0:
         raise _lib.NeurayB200Error(f"MVSNet: unsupported shape (images {h}x{w}, {sn} depth planes: h/4, w/4 and the planes must be multiples of 8)")
-    ws = encoders._workspace("mvsnet", nbytes, dev)
+    ws = _lib.workspace("mvsnet", nbytes, dev, torch.uint8)
     prob = torch.empty(rfn, ho.value, wo.value, sn, dtype=torch.float32, device=dev)
     depth = torch.empty(rfn, ho.value, wo.value, dtype=torch.float32, device=dev)
     with _lib.on_device(imgs):
@@ -259,7 +259,7 @@ def cost_volume_forward_into(module, ref_imgs_info, src_imgs_info, is_train, out
     depth_norm = extract_depth_for_init({"depth": depth[:, None], "depth_range": ref_imgs_info["depth_range"]})
     packed = _packed_cv(module, "head", sn, dev)
     nbytes = _lib.lib().nr_cost_volume_head_workspace(sn, rfn, h, w)
-    ws = encoders._workspace("cv_head", nbytes, dev)
+    ws = _lib.workspace("cv_head", nbytes, dev, torch.uint8)
     x = imgs.detach().contiguous().float()
     with _lib.on_device(imgs):
         _lib.check(_lib.lib().nr_cost_volume_head_fwd(sn, _lib.ptr(packed), _lib.ptr(x), _lib.ptr(prob), _lib.ptr(depth_norm), rfn, h, w, _lib.ptr(out),

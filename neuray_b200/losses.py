@@ -81,7 +81,7 @@ def gen_depth_loss_coords(h, w, num, device):
 def predict_mean_for_depth_loss(self, ref_imgs_info):
     """NeuralRayGenRenderer.predict_mean_for_depth_loss (renderer.py:280-316) for an owner with dist_decoder
     (/ fine_dist_decoder) under the reference's parameter names; returns the same dict."""
-    from .renderer import pass_index_map, pass_weights
+    from .renderer import pass_index_map, pass_params, pass_weights
     ray_feats, ref_imgs = ref_imgs_info["ray_feats"], ref_imgs_info["imgs"]
     if not ray_feats.is_cuda:
         raise _lib.NeurayB200Error("predict_mean_for_depth_loss needs CUDA tensors (no CPU fallback)")
@@ -89,18 +89,18 @@ def predict_mean_for_depth_loss(self, ref_imgs_info):
     coords = gen_depth_loss_coords(h, w, self.cfg["depth_loss_coords_num"], ref_imgs.device)
     coords = coords.unsqueeze(0).repeat(rfn, 1, 1)
     fine = bool(self.cfg["use_hierarchical_sampling"])
-    decs = [("dist_decoder", self.dist_decoder, False)] + ([("fine_dist_decoder", self.fine_dist_decoder, True)] if fine else [])
     w_point, names, index_maps, params, param_names = [], [], [], [], []
-    for dec_name, dec, is_fine in decs:
+    for is_fine in ((False, True) if fine else (False,)):
+        pp = pass_params(self, is_fine)
         dn = self.cfg["fine_depth_sample_num" if is_fine else "depth_sample_num"]
         if is_fine and self.cfg["fine_depth_use_all"]:
             dn += self.cfg["depth_sample_num"]
         w_point.append(pass_weights(self, is_fine, dn, ray_feats.device)[0])
-        own = {f"{dec_name}.{k}": v for k, v in dec.named_parameters() if k.startswith("mean_decoder.")}
-        index_maps.append(pass_index_map(self, is_fine, ray_feats.device))     # covers the whole pass; only the mean head gets a gradient here
-        names.append(list(own))
-        params += list(own.values())
-        param_names += list(own)
+        own = [(n, v) for n, v in pp.named if n.startswith(f"{pp.dec_name}.mean_decoder.")]
+        index_maps.append(pass_index_map(self, pp, ray_feats.device))     # covers the whole pass; only the mean head gets a gradient here
+        names.append([n for n, _ in own])
+        params += [v for _, v in own]
+        param_names += names[-1]
     meta = {"coords": coords.float().contiguous(), "h": h, "w": w, "w_point": w_point, "names": names, "index_maps": index_maps,
             "param_names": param_names}
     means = _DepthMeanFn.apply(meta, ray_feats, *params)

@@ -9,7 +9,7 @@ checkpoint loads unchanged -- the state-dict key names and shapes are the compat
     MultiHeadAttention            reference network/ibrnet.py:52-72
 
 They hold parameters only.  There is deliberately no torch `forward`: the arithmetic runs in the CUDA
-kernels (neuray_b200/csrc), fed by `neuray_b200.weights.pack_pass_weights`.
+kernels (neuray_b200/csrc).
 """
 import torch
 import torch.nn as nn

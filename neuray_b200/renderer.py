@@ -17,6 +17,8 @@ The functions below are written against "owner": any nn.Module that has `.cfg` (
 sub-modules dist_decoder / agg_net (/ fine_dist_decoder / fine_agg_net) with the reference's parameter names.
 """
 import ctypes as C
+from dataclasses import dataclass
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -63,24 +65,6 @@ def set_precision(mode):
     if mode not in ("fp32", "tf32"):
         raise ValueError(f"render precision {mode!r}: 'fp32' or 'tf32'")
     PRECISION = mode
-
-
-# Grow-only device workspaces, reused across passes, chunks and frames.  The C-ABI never allocates (the caller owns
-# the workspace); taking 335 MB of point records per pass and 246 MB of repacked maps per frame from torch's caching
-# allocator every time fragmented it (small long-lived outputs land in the freed big blocks) and cost cudaMalloc calls
-# in steady state (tools/e2e_breakdown.py).  Everything is stream-ordered on the caller's current stream; rendering
-# with one network object from several streams at once is not supported.
-_WORKSPACES = {}
-
-
-def _workspace(key, numel, dev):
-    buf = _WORKSPACES.get((key, str(dev)))
-    if buf is None or buf.numel() < numel:
-        buf = None
-        _WORKSPACES.pop((key, str(dev)), None)
-        buf = torch.empty(numel, dtype=torch.float32, device=dev)
-        _WORKSPACES[(key, str(dev))] = buf
-    return buf[:numel]
 
 
 _PACK_POOL = {}      # (device, feat shape, rgb shape) -> [(feat, rgb)] of dropped FramePacks, at most two kept
@@ -168,55 +152,72 @@ def frame_pack(ref_imgs_info):
     return pack
 
 
-def _pass_modules(owner, is_fine):
-    return (owner.fine_dist_decoder, owner.fine_agg_net, "fine_dist_decoder", "fine_agg_net") if is_fine else \
-        (owner.dist_decoder, owner.agg_net, "dist_decoder", "agg_net")
+class PassParams(NamedTuple):
+    """One pass' modules, their state-dict prefixes and its parameters as [(state-dict name, tensor)]: the decoder's
+    named_parameters(), then the aggregation net's.  backward.RenderPassFn and backward.layer_table read the gradients
+    by these names in this order."""
+    is_fine: bool
+    dec: nn.Module
+    agg: nn.Module
+    dec_name: str
+    agg_name: str
+    named: list
+
+
+def pass_params(owner, is_fine):
+    dec_name, agg_name = ("fine_dist_decoder", "fine_agg_net") if is_fine else ("dist_decoder", "agg_net")
+    dec, agg = getattr(owner, dec_name), getattr(owner, agg_name)
+    named = [(f"{dec_name}.{k}", v) for k, v in dec.named_parameters()] + [(f"{agg_name}.{k}", v) for k, v in agg.named_parameters()]
+    return PassParams(is_fine, dec, agg, dec_name, agg_name, named)
+
+
+@dataclass
+class _PackedPass:
+    """The owner's cache entry of one pass' packed weights."""
+    stamp: tuple            # (data_ptr, _version) of every parameter, then the device packed for
+    w_point: torch.Tensor   # nr_pack_weights' buffers: fresh on every re-pack
+    w_ray: torch.Tensor
+    w_tc: torch.Tensor
+    pos_enc: dict           # dn -> posenc table on the device; kept across re-packs
+    w_tc_tf32: torch.Tensor = None      # nr_pack_weights_tf32's w_tc, made on first use after each re-pack
 
 
 def pass_weights(owner, is_fine, dn, device, tf32=False):
-    """Packed weights of one pass (nr_pack_weights), cached on the owner and re-packed when any parameter changed
-    (optimizer steps bump tensor._version).  Every re-pack gets fresh buffers: an autograd graph recorded before the
-    parameter update keeps reading the buffers it was recorded with.  tf32: w_tc is the TF32 mode's pack
+    """(w_point, w_ray, pos_enc, w_tc) of one pass (nr_pack_weights), cached on the owner and re-packed when any parameter
+    changed (optimizer steps bump tensor._version).  Every re-pack gets fresh buffers: an autograd graph recorded before
+    the parameter update keeps reading the buffers it was recorded with.  tf32: w_tc is the TF32 mode's pack
     (nr_pack_weights_tf32), made on first use after each re-pack and cached next to the other one."""
-    dec, agg, dec_name, agg_name = _pass_modules(owner, is_fine)
-    params = {f"{dec_name}.{k}": v for k, v in dec.named_parameters()}
-    params.update({f"{agg_name}.{k}": v for k, v in agg.named_parameters()})
+    pp = pass_params(owner, is_fine)
+    params = dict(pp.named)
     stamp = tuple((v.data_ptr(), v._version) for v in params.values()) + (str(device),)
     cache = owner.__dict__.setdefault("_nr_wcache", {})
-    hit = cache.get(is_fine)
-    if hit is None or hit[0] != stamp:
-        first = next(iter(params.values()))
+    entry = cache.get(is_fine)
+    if entry is None or entry.stamp != stamp:
+        first = pp.named[0][1]
         if first.device != torch.device(device):
             raise _lib.NeurayB200Error(f"parameters live on {first.device} but the rays are on {device}")
-        wp, wr, wt = pack_pass(params, dec_name, agg_name)
-        hit = (stamp, wp, wr, hit[3] if hit is not None else {}, wt, {})
-        cache[is_fine] = hit
-    pe = hit[3].get(dn)
+        w_point, w_ray, w_tc = pack_pass(params, pp.dec_name, pp.agg_name)
+        pos_enc = entry.pos_enc if entry is not None else {}
+        entry = cache[is_fine] = _PackedPass(stamp, w_point, w_ray, w_tc, pos_enc)
+    pe = entry.pos_enc.get(dn)
     if pe is None:
-        n_samples = agg.agg_impl.n_samples
+        n_samples = pp.agg.agg_impl.n_samples
         if n_samples != dn:
             # the reference fails with a broadcast error here (ibrnet.py:356); keep that behaviour explicit
             raise _lib.NeurayB200Error(
-                f"{agg_name}: pos_encoding was built for sample_num={n_samples} but the pass has {dn} samples per ray")
-        pe = posenc_table(dn).to(device).contiguous()
-        hit[3][dn] = pe
-    if not tf32:
-        return hit[1], hit[2], pe, hit[4]
-    wt = hit[5].get("tf32")
-    if wt is None:
-        wt = hit[5]["tf32"] = pack_pass_tf32(params, dec_name, agg_name)
-    return hit[1], hit[2], pe, wt
+                f"{pp.agg_name}: pos_encoding was built for sample_num={n_samples} but the pass has {dn} samples per ray")
+        pe = entry.pos_enc[dn] = posenc_table(dn).to(device).contiguous()
+    if tf32 and entry.w_tc_tf32 is None:
+        entry.w_tc_tf32 = pack_pass_tf32(params, pp.dec_name, pp.agg_name)
+    return entry.w_point, entry.w_ray, pe, entry.w_tc_tf32 if tf32 else entry.w_tc
 
 
-def pass_index_map(owner, is_fine, dev):
-    """weights.point_index_map of a pass (packed w_point position -> parameter element), cached on the owner."""
-    dec, agg, dec_name, agg_name = _pass_modules(owner, is_fine)
-    allp = {f"{dec_name}.{k}": v for k, v in dec.named_parameters()}
-    allp.update({f"{agg_name}.{k}": v for k, v in agg.named_parameters()})
+def pass_index_map(owner, pp, dev):
+    """weights.point_index_map of the pass pp (packed w_point position -> parameter element), cached on the owner."""
     maps = owner.__dict__.setdefault("_nr_index_maps", {})
-    key = (is_fine, str(dev), tuple(allp))
+    key = (pp.is_fine, str(dev), tuple(n for n, _ in pp.named))
     if key not in maps:
-        maps[key] = point_index_map(allp, dec_name, agg_name)
+        maps[key] = point_index_map(dict(pp.named), pp.dec_name, pp.agg_name)
     return maps[key]
 
 
@@ -240,52 +241,59 @@ def _sh_regs(owner):
     return hit[1]
 
 
-def _direct_render(owner, out, rn, dn, dev):
-    """use_dr_prediction (reference renderer.py:85-125, 181-185): nr_direct_render enqueued right behind the pass whose raw
-    outputs `out` holds, while that pass' point record is still in the shared workspace.  Returns pixel_colors_dr [1,rn,3]
-    and hit_prob_dr [1,rn,dn]."""
+def _direct_render(owner, launch, rn, dn, dev):
+    """use_dr_prediction (reference renderer.py:85-125, 181-185): nr_direct_render enqueued right behind the pass `launch`
+    describes, while that pass' point record is still in the shared workspace.  Returns pixel_colors_dr [1,rn,3] and
+    hit_prob_dr [1,rn,dn]."""
     res = {"pixel_colors_dr": torch.empty(1, rn, 3, dtype=torch.float32, device=dev),
            "hit_prob_dr": torch.empty(1, rn, dn, dtype=torch.float32, device=dev)}
-    if out["_bwd"] is None:          # rn == 0: nothing was launched
+    if launch is None:          # rn == 0: nothing was launched
         return res
-    p, _keep, _, stream = out["_bwd"]
     d = _lib.NrDrParams()
     d.regs[:] = _sh_regs(owner)
     d.alpha_ground_state = float(owner.cfg["alpha_value_ground_state"])
     d.use_nr_color = 1 if owner.cfg["use_nr_color_for_dr"] else 0
-    d.point_colors = _lib.ptr(_workspace("dr_point_colors", rn * dn * 3, dev))
+    d.point_colors = _lib.ptr(_lib.workspace("dr_point_colors", rn * dn * 3, dev))
     d.pixel_colors_dr, d.hit_prob_dr = _lib.ptr(res["pixel_colors_dr"]), _lib.ptr(res["hit_prob_dr"])
     with _lib.on_device(res["hit_prob_dr"]):
-        _lib.check(_lib.lib().nr_direct_render(C.byref(p), C.byref(d), stream), "nr_direct_render")
+        _lib.check(_lib.lib().nr_direct_render(C.byref(launch.params), C.byref(d), launch.stream), "nr_direct_render")
     _lib.count_launches(2)
     return res
 
 
-def _view_visibility(out, rn, rfn, dev):
-    """render_visibility: nr_view_visibility enqueued right behind the pass whose raw outputs `out` holds, on its
-    hit_prob.  Returns visibility [1,rn,rfn]: Σ_d hit_prob · the masked prj_dict['vis'] of each view (renderer.py:79-82)."""
+def _view_visibility(launch, hit_prob, rn, rfn, dev):
+    """render_visibility: nr_view_visibility enqueued right behind the pass `launch` describes, on its hit_prob.  Returns
+    visibility [1,rn,rfn]: Σ_d hit_prob · the masked prj_dict['vis'] of each view (renderer.py:79-82)."""
     vis = torch.empty(1, rn, rfn, dtype=torch.float32, device=dev)
-    if out["_bwd"] is None:          # rn == 0: nothing was launched
+    if launch is None:          # rn == 0: nothing was launched
         return vis
-    p, _keep, _, stream = out["_bwd"]
     q = _lib.NrVisParams()
-    q.hit_prob, q.visibility = _lib.ptr(out["hit_prob"]), _lib.ptr(vis)
+    q.hit_prob, q.visibility = _lib.ptr(hit_prob), _lib.ptr(vis)
     with _lib.on_device(vis):
-        _lib.check(_lib.lib().nr_view_visibility(C.byref(p), C.byref(q), stream), "nr_view_visibility")
+        _lib.check(_lib.lib().nr_view_visibility(C.byref(launch.params), C.byref(q), launch.stream), "nr_view_visibility")
     _lib.count_launches(1)
     return vis
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit, tf32=False):
-    """Enqueues the two kernels of one pass; returns the raw output dict (ray_mask as uint8).  tf32: the point kernel in
-    TF32 mode (set_precision)."""
+class PassLaunch(NamedTuple):
+    """A launched pass, for what runs on the same inputs after it: direct rendering, visibility and nr_render_pass_bwd
+    (the autograd node keeps it alive; otherwise it is dropped with the pass' outputs)."""
+    params: _lib.NrPassParams
+    keep: tuple             # the tensors params points into
+    feat_shape: tuple       # [rfn,fh,fw,64] of the channel-last feature-map gradient
+    stream: int
+
+
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32):
+    """Enqueues the two kernels of the pass pp; returns its raw outputs (ray_mask as uint8) and its PassLaunch, None when
+    there are no rays.  tf32: the point kernel in TF32 mode (set_precision)."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
     pack = frame_pack(ref_imgs_info)
     _, rn, dn = que_depth.shape
-    dec, agg, _, _ = _pass_modules(owner, is_fine)
-    w_point, w_ray, pos_enc, w_tc = pass_weights(owner, is_fine, dn, dev, tf32)
+    dec = pp.dec
+    w_point, w_ray, pos_enc, w_tc = pass_weights(owner, pp.is_fine, dn, dev, tf32)
     cam = que_imgs_info.get(CAM_KEY)
     if cam is None:
         cam, _ = camera_blocks(que_imgs_info, None)
@@ -297,7 +305,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
         "render_depth": torch.empty(1, rn, dtype=torch.float32, device=dev),
         "ray_mask_u8": torch.empty(1, rn, dtype=torch.uint8, device=dev),
     }
-    rec = _workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
+    rec = _lib.workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
     p = _lib.NrPassParams()
     p.coords, p.que_depth, p.que_cam = _lib.ptr(coords_c), _lib.ptr(que_depth), _lib.ptr(cam)
     p.rn, p.dn = rn, dn
@@ -321,8 +329,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
         p.fine_u, p.fine_u_stride, p.fine_depth = _lib.ptr(fine["u"]), int(fine["u_stride"]), _lib.ptr(out["fine_depth"])
     stream = _lib.stream_of(coords)
     if rn == 0:          # nothing to render: the (empty) outputs are already in place
-        out["_bwd"] = None
-        return out
+        return out, None
     with _lib.on_device(coords):
         if _lib.PROFILE is not None:
             # bench.py: time the dominant kernel alone, with CUDA events on the launching stream
@@ -341,9 +348,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, 
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
     _lib.count_launches(2)
-    # what nr_render_pass_bwd needs to run on the same inputs (kept alive by the autograd node, dropped otherwise)
-    out["_bwd"] = (p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
-    return out
+    return out, PassLaunch(p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
 
 
 def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None, want_hit=True):
@@ -363,62 +368,48 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     _, rn, dn = que_depth.shape
     if dn > _lib.NR_MAX_SAMPLES:
         raise _lib.NeurayB200Error(f"at most {_lib.NR_MAX_SAMPLES} samples per ray per pass, got {dn}")
-    dec, agg, dec_name, agg_name = _pass_modules(owner, is_fine)
+    pp = pass_params(owner, is_fine)
     rf, imf = ref_imgs_info["ray_feats"], ref_imgs_info["img_feats"]
-    named = [(f"{dec_name}.{k}", v) for k, v in dec.named_parameters()] + [(f"{agg_name}.{k}", v) for k, v in agg.named_parameters()]
-    needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for _, v in named))
-    dr = {} if owner.cfg["use_dr_prediction"] else None
-    vis = {} if owner.cfg.get("render_visibility", False) else None
-    tf32 = PRECISION == "tf32" and not needs_grad
-
-    def launch():
-        out = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine, want_hit or vis is not None, tf32)
+    params = [v for _, v in pp.named]
+    needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for v in params))
+    want_dr, want_vis = owner.cfg["use_dr_prediction"], owner.cfg.get("render_visibility", False)
+    out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit or want_vis,
+                               PRECISION == "tf32" and not needs_grad)
+    dr = _direct_render(owner, launch, rn, dn, coords.device) if want_dr else None
+    if want_vis:
+        out["visibility"] = _view_visibility(launch, out["hit_prob"], rn, rf.shape[0], coords.device)
+    if needs_grad:
+        from .backward import DirectRenderFn, RenderPassFn
+        meta = {"names": [n for n, _ in pp.named], "dec": pp.dec_name, "agg": pp.agg_name}
+        res = RenderPassFn.apply(launch, out, meta, rf, imf, *params)
+        out.update(zip(("pixel_colors", "hit_prob", "render_depth", "ray_mask_u8", "fine_depth"), res))
         if dr is not None:
-            dr.update(_direct_render(owner, out, rn, dn, coords.device))
-        if vis is not None:
-            vis["visibility"] = _view_visibility(out, rn, rf.shape[0], coords.device)
-        return out
-    if not needs_grad:
-        out = launch()
-        out.pop("_bwd", None)
-    else:
-        from .backward import RenderPassFn
-        meta = {"names": [n for n, _ in named], "dec": dec_name, "agg": agg_name}
-        res = RenderPassFn.apply(launch, meta, rf, imf, *[v for _, v in named])
-        out = {"pixel_colors": res[0], "hit_prob": res[1], "render_depth": res[2], "ray_mask_u8": res[3]}
-        if fine:
-            out["fine_depth"] = res[4]
-        if dr is not None:
-            from .backward import DirectRenderFn
-            dr = dict(zip(("pixel_colors_dr", "hit_prob_dr"), DirectRenderFn.apply(dr, rf, imf, *[v for _, v in named])))
+            dr = dict(zip(("pixel_colors_dr", "hit_prob_dr"), DirectRenderFn.apply(dr, rf, imf, *params)))
     if dr is not None:
         out.update(dr)
-    if vis is not None:
-        out.update(vis)
     out["ray_mask"] = out.pop("ray_mask_u8").bool()
     return out
 
 
-def _finish_outputs(owner, res, que_depth, que_imgs_info):
-    cfg = owner.cfg
+# the optional outputs of a pass: (cfg switch, run_pass key, output key)
+_OPTIONAL_OUTPUTS = (("use_dr_prediction", "pixel_colors_dr", "pixel_colors_dr"), ("use_dr_prediction", "hit_prob_dr", "hit_prob_dr"),
+                     ("use_ray_mask", "ray_mask", "ray_mask"), ("render_depth", "render_depth", "render_depth"),
+                     ("render_visibility", "visibility", "visibility_nr"))
+
+
+def _finish_outputs(owner, res, que_imgs_info):
     outputs = {"pixel_colors_nr": res["pixel_colors"], "hit_prob_nr": res["hit_prob"]}
-    if cfg["use_dr_prediction"]:
-        outputs["pixel_colors_dr"], outputs["hit_prob_dr"] = res["pixel_colors_dr"], res["hit_prob_dr"]
     if "imgs" in que_imgs_info:
         outputs["pixel_colors_gt"] = interpolate_feats(que_imgs_info["imgs"], que_imgs_info["coords"], align_corners=True)
-    if cfg["use_ray_mask"]:
-        outputs["ray_mask"] = res["ray_mask"]
-    if cfg["render_depth"]:
-        outputs["render_depth"] = res["render_depth"]
-    if cfg.get("render_visibility", False):
-        outputs["visibility_nr"] = res["visibility"]
+    outputs.update((key, res[raw]) for switch, raw, key in _OPTIONAL_OUTPUTS if owner.cfg.get(switch, False))
     return outputs
 
 
 def _self_hit_prob(self, que_depth, que_imgs_info, is_fine):
     """a17 predict_self_hit_prob (reference renderer.py:137-155): the query view's own ray_feats decoded along its rays
     (fine-tuning configs).  nr_self_hit_prob, forward and backward."""
-    dec, _, dec_name, _ = _pass_modules(self, is_fine)
+    pp = pass_params(self, is_fine)
+    dec = pp.dec
     feats = que_imgs_info["ray_feats"]
     coords = que_imgs_info["coords"]
     h, w = que_imgs_info["imgs"].shape[-2:]
@@ -428,8 +419,7 @@ def _self_hit_prob(self, que_depth, que_imgs_info, is_fine):
     dev = coords.device
     _, rn, dn = que_depth.shape
     w_point = pass_weights(self, is_fine, dn, dev)[0]
-    dec_params = {f"{dec_name}.{k}": v for k, v in dec.named_parameters()}
-    index_map = pass_index_map(self, is_fine, dev)
+    index_map = pass_index_map(self, pp, dev)
     fmap = feats[0].detach().contiguous().float()
     cc, qd = coords[0].detach().contiguous().float(), que_depth[0].detach().contiguous().float()
     rng = que_imgs_info["depth_range"][0].detach().float().contiguous()
@@ -442,7 +432,7 @@ def _self_hit_prob(self, que_depth, que_imgs_info, is_fine):
         p.depth_range, p.var_bias = _lib.ptr(rng), var_bias
         return p
 
-    named = list(dec_params.items())
+    named = [(n, v) for n, v in pp.named if n.startswith(pp.dec_name + ".")]
     meta = {"params": params, "index_map": index_map, "stream": _lib.stream_of(coords), "map_shape": tuple(fmap.shape),
             "dec_names": [n for n, _ in named], "keep": (fmap, cc, qd, w_point, rng)}
     return SelfHitProbFn.apply(meta, feats, *[v for _, v in named])
@@ -451,7 +441,7 @@ def _self_hit_prob(self, que_depth, que_imgs_info, is_fine):
 def render_by_depth(self, que_depth, que_imgs_info, ref_imgs_info, is_train, is_fine):
     """reference renderer.py:168-203."""
     res = run_pass(self, que_depth, que_imgs_info, ref_imgs_info, is_fine)
-    outputs = _finish_outputs(self, res, que_depth, que_imgs_info)
+    outputs = _finish_outputs(self, res, que_imgs_info)
     if is_train and self.cfg["use_self_hit_prob"]:
         outputs["hit_prob_self"] = _self_hit_prob(self, que_depth, que_imgs_info, is_fine)
     return outputs
@@ -484,13 +474,13 @@ def render_impl(self, que_imgs_info, ref_imgs_info, is_train):
     rn = que_imgs_info["coords"].shape[1]
     fine = _fine_request(self, rn, is_train, que_depth.device) if hier else None
     res = run_pass(self, que_depth, que_imgs_info, ref_imgs_info, False, fine=fine)
-    outputs = _finish_outputs(self, res, que_depth, que_imgs_info)
+    outputs = _finish_outputs(self, res, que_imgs_info)
     self_hit = is_train and self.cfg["use_self_hit_prob"]
     if self_hit:
         outputs["hit_prob_self"] = _self_hit_prob(self, que_depth, que_imgs_info, False)
     if hier:
         res_f = run_pass(self, res["fine_depth"], que_imgs_info, ref_imgs_info, True)
-        fine_out = _finish_outputs(self, res_f, res["fine_depth"], que_imgs_info)
+        fine_out = _finish_outputs(self, res_f, que_imgs_info)
         if self_hit:
             fine_out["hit_prob_self"] = _self_hit_prob(self, res["fine_depth"], que_imgs_info, True)
         for k, v in fine_out.items():
