@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 11
+#define NR_ABI_VERSION 12
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -196,6 +196,22 @@ typedef struct NrVisParams {
   float* visibility;         /* [rn,rfn] */
 } NrVisParams;
 int nr_view_visibility(const NrPassParams* p, const NrVisParams* v, void* stream);
+
+/* Per-view colour-blend weight of each rendered pixel (cfg render_blend_weights): nr_render_pass_fwd (or _tf32) with the
+ * point kernel also exporting each (view, point) row's blend weight w, then one reduction kernel:
+ *   blend_weights[r, v] = Σ_d hit_prob[r, d] · w[v, r, d]
+ * w is the reference's blending_weights_valid of the same pass (ibrnet.py:362-366: softmax over the views of rgb_fc's
+ * logit, set to -1e9 where the projection mask is 0; a point no view sees gets 1/rfn from every view), hit_prob the pass'
+ * compositing weight (hit_prob_nr, so p->hit_prob is required).  Views in view_params order; unnormalised, like
+ * render_depth: Σ_v blend_weights[r, v] = Σ_d hit_prob[r, d].  Each ray's sum runs in an order fixed by dn alone, so a ray's
+ * result does not depend on the chunk or launch that renders it.  Every other output equals the one of the twin without
+ * _blend bit for bit.  Three kernels, no host synchronisation. */
+typedef struct NrBlendParams {
+  float* row_blend;          /* workspace [rfn, rn*dn] */
+  float* blend_weights;      /* [rn,rfn] */
+} NrBlendParams;
+int nr_render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);
+int nr_render_pass_fwd_tf32_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);   /* TF32 mode */
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);

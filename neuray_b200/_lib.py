@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -52,6 +52,10 @@ class NrVisParams(C.Structure):
     _fields_ = [("hit_prob", C.c_void_p), ("visibility", C.c_void_p)]
 
 
+class NrBlendParams(C.Structure):
+    _fields_ = [("row_blend", C.c_void_p), ("blend_weights", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -83,6 +87,8 @@ SIGNATURES = {
     "nr_render_pass_fwd_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_direct_render": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrDrParams), _vp]),
     "nr_view_visibility": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrVisParams), _vp]),
+    "nr_render_pass_fwd_blend": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrBlendParams), _vp]),
+    "nr_render_pass_fwd_tf32_blend": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrBlendParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),

@@ -229,9 +229,27 @@ __global__ void fine_depth_kernel(const float* __restrict__ depth, const float* 
 
 }  // namespace ops
 
-// implemented in nr_point_kernel.cu / nr_ray_kernel.cu
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, bool tf32, cudaStream_t stream);
+// implemented in nr_point_kernel.cu / nr_ray_kernel.cu / nr_blend.cu
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* row_blend, bool tf32, cudaStream_t stream);
 int launch_ray_kernel(const NrPassParams* p, cudaStream_t stream);
+int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, cudaStream_t stream);
+
+// One render pass: the point kernel (3xTF32 or TF32 mode; row_blend: optional export of its colour-blend weights), then
+// the ray kernel.  Every nr_render_pass_fwd* entry point is this sequence.
+static int render_pass_fwd(const NrPassParams* p, float* row_blend, bool tf32, cudaStream_t stream) {
+  const int rc = launch_point_kernel(p, nullptr, nullptr, row_blend, tf32, stream);
+  if (rc != NR_OK) return rc;
+  return launch_ray_kernel(p, stream);
+}
+
+// The pass with the blend-weight export on, then the reduction over its hit_prob.
+static int render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, bool tf32, cudaStream_t stream) {
+  NR_CHECK_ARG(p != nullptr && b != nullptr, "params");
+  if (p->rn > 0) NR_CHECK_ARG(b->row_blend && b->blend_weights && p->hit_prob, "null blend workspace, blend_weights or hit_prob");
+  const int rc = render_pass_fwd(p, b->row_blend, tf32, stream);
+  if (rc != NR_OK) return rc;
+  return launch_blend_weights(p, b, stream);
+}
 
 static thread_local char g_err[512] = "";
 void set_error(const char* fmt, ...) {
@@ -294,26 +312,24 @@ int nr_pack_feature_maps(const float* ray_feats, const float* img_feats, const f
   return NR_OK;
 }
 
-int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, false, (cudaStream_t)stream); }
-int nr_point_kernel_tf32(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, true, (cudaStream_t)stream); }
+int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, false, (cudaStream_t)stream); }
+int nr_point_kernel_tf32(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, true, (cudaStream_t)stream); }
 int nr_point_kernel_debug(const NrPassParams* p, float* dbg, void* stream) {
   NR_CHECK_ARG(dbg != nullptr, "dbg");
-  return launch_point_kernel(p, dbg, nullptr, false, (cudaStream_t)stream);
+  return launch_point_kernel(p, dbg, nullptr, nullptr, false, (cudaStream_t)stream);
 }
 int nr_point_kernel_timing(const NrPassParams* p, long long* timing, void* stream) {
   NR_CHECK_ARG(timing != nullptr && p != nullptr && p->w_tc != nullptr, "timing buffer / tensor-core weights required");
-  return launch_point_kernel(p, nullptr, timing, false, (cudaStream_t)stream);
+  return launch_point_kernel(p, nullptr, timing, nullptr, false, (cudaStream_t)stream);
 }
 int nr_ray_kernel(const NrPassParams* p, void* stream) { return launch_ray_kernel(p, (cudaStream_t)stream); }
-int nr_render_pass_fwd(const NrPassParams* p, void* stream) {
-  const int rc = launch_point_kernel(p, nullptr, nullptr, false, (cudaStream_t)stream);
-  if (rc != NR_OK) return rc;
-  return launch_ray_kernel(p, (cudaStream_t)stream);
+int nr_render_pass_fwd(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, false, (cudaStream_t)stream); }
+int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, true, (cudaStream_t)stream); }
+int nr_render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, void* stream) {
+  return render_pass_fwd_blend(p, b, false, (cudaStream_t)stream);
 }
-int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream) {
-  const int rc = launch_point_kernel(p, nullptr, nullptr, true, (cudaStream_t)stream);
-  if (rc != NR_OK) return rc;
-  return launch_ray_kernel(p, (cudaStream_t)stream);
+int nr_render_pass_fwd_tf32_blend(const NrPassParams* p, const NrBlendParams* b, void* stream) {
+  return render_pass_fwd_blend(p, b, true, (cudaStream_t)stream);
 }
 
 int nr_sample_depth(const float* depth_range, int rn, int dn, const float* jitter, float* depth, float* dists, void* stream) {

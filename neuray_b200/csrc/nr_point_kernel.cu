@@ -43,6 +43,7 @@ struct KParams {
   NrPassParams p;
   float* dbg;
   long long* timing;   // optional: clock64() at phase boundaries, CTA 0, thread 0 of each compute warp group: [tile][2][32]
+  float* row_blend;    // optional: each valid (view, point) row's colour-blend weight, [rfn][rn*dn] (warp group 1, end of tile)
   int P, n_tiles, n_heads;
 };
 
@@ -310,19 +311,21 @@ static int device_sms() {
 // The dynamic shared-memory opt-in is a per-device function attribute; it is set on every launch (a few hundred
 // nanoseconds against a kernel of milliseconds) so that the library keeps no per-process state: a process may render on
 // any number of devices from any number of threads.
-// TF32: the TF32-mode kernel (release form only), else the 3xTF32 one
-template <int G, bool DEBUG, bool TF32>
+// TF32: the TF32-mode kernel (release form only), else the 3xTF32 one; BLEND: the release form with the colour-blend
+// export (kp.row_blend)
+template <int G, bool DEBUG, bool TF32, bool BLEND = false>
 static int launch_pm3_inst(const pkt::KParams& kp, int grid, cudaStream_t stream) {
-  static_assert(!(TF32 && DEBUG), "the TF32 mode has no debug form");
+  static_assert(!(TF32 && DEBUG) && !(BLEND && DEBUG), "the TF32 mode and the blend export have no debug form");
   void (*fn)(const pkt::KParams);
-  if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
+  if constexpr (BLEND) fn = pkt::pm3::point_kernel_blend<G, TF32 ? 1 : 3>;
+  else if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
   else fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
   if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(pkt::pm3::SMEM_BYTES)) != cudaSuccess) {
     nr::set_error("point kernel: cannot opt in to %zu bytes of shared memory: %s", pkt::pm3::SMEM_BYTES, cudaGetErrorString(cudaGetLastError()));
     return NR_E_CUDA;
   }
   fn<<<grid, pkt::pm3::NTHR, pkt::pm3::SMEM_BYTES, stream>>>(kp);
-  NR_CHECK_LAUNCH(TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
+  NR_CHECK_LAUNCH(BLEND ? "point_kernel_blend" : TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
   return NR_OK;
 }
 
@@ -334,15 +337,19 @@ static int launch_pm3(pkt::KParams kp, bool tf32, cudaStream_t stream) {
   kp.n_tiles = int((N + PB - 1) / PB);
   const int sms = device_sms();
   const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
+  if (kp.row_blend)
+    return tf32 ? launch_pm3_inst<G, false, true, true>(kp, grid, stream) : launch_pm3_inst<G, false, false, true>(kp, grid, stream);
   if (tf32) return launch_pm3_inst<G, false, true>(kp, grid, stream);
   return (kp.dbg || kp.timing) ? launch_pm3_inst<G, true, false>(kp, grid, stream) : launch_pm3_inst<G, false, false>(kp, grid, stream);
 }
 
 // `timing`: optional clock64() stamps at the phase boundaries (nr_point_kernel_timing), passed per call.  tf32: the TF32
-// mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, bool tf32, cudaStream_t stream) {
+// mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.  row_blend: optional
+// [rfn][rn*dn] export of the colour-blend weights (nr_render_pass_fwd_blend / _tf32_blend), in either mode.
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* row_blend, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr, "params");
   NR_CHECK_ARG(!tf32 || (dbg == nullptr && timing == nullptr), "the TF32 point kernel has no debug tap or phase stamps");
+  NR_CHECK_ARG(!row_blend || (dbg == nullptr && timing == nullptr), "the blend export has no debug tap or phase stamps");
   NR_CHECK_ARG(p->coords && p->que_depth && p->que_cam && p->feat && p->rgb && p->view_params && p->w_point && p->point_rec,
                "null device pointer");
   NR_CHECK_ARG(p->w_tc != nullptr, "w_tc (tensor-core weight buffer, nr_pack_weights) is required");
@@ -357,6 +364,7 @@ int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, bo
   kp.p = *p;
   kp.dbg = dbg;
   kp.timing = timing;
+  kp.row_blend = row_blend;
   kp.n_heads = p->use_vis ? 4 : 3;
   // lanes per point: the smallest group size that holds the views and wastes the fewest of a warp's 32 lanes
   if (p->rfn <= 4) return launch_pm3<4>(kp, tf32, stream);

@@ -521,8 +521,10 @@ __device__ __forceinline__ void ld_row(const Blk& b, int col, float* v) {
   }
 }
 
-// The kernel body, NP passes per tensor-core product (point_kernel_pm3: 3, point_kernel_tf32: 1)
-template <int G, bool DEBUG, int NP>
+// The kernel body, NP passes per tensor-core product (point_kernel_pm3: 3, point_kernel_tf32: 1).  BLEND: warp group 1
+// also stores each valid row's colour-blend weight into kp.row_blend (point_kernel_blend); a compile-time switch, so that
+// the kernels without the export are the same code as before it existed.
+template <int G, bool DEBUG, int NP, bool BLEND = false>
 __device__ __forceinline__ void point_body(const KParams& kp) {
   extern __shared__ __align__(1024) float smem[];
   constexpr bool P2 = (G & (G - 1)) == 0;      // power-of-two lane groups reduce with butterflies, the others through shared memory
@@ -1185,6 +1187,10 @@ __device__ __forceinline__ void point_body(const KParams& kp) {
         float4* __restrict__ dst = reinterpret_cast<float4*>(pp.point_rec + size_t(n) * REC);
         dst[4] = make_float4(acc[1] / acc[0], acc[2] / acc[0], acc[3] / acc[0], msum);
       }
+      // the blend weight of this (view, point) row (nr_render_pass_fwd_blend): the reference's blending_weights_valid
+      if constexpr (BLEND) {
+        if (row_ok) kp.row_blend[size_t(v) * N + n] = e / acc[0];
+      }
     }
     PM_TICK(15)
   }
@@ -1197,5 +1203,8 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) { 
 // rna(W) in the hi slots (nr_pack_weights_tf32)
 template <int G>
 __global__ void __launch_bounds__(NTHR, 1) point_kernel_tf32(const KParams kp) { point_body<G, false, 1>(kp); }
+// Either release form (NP = 3: 3xTF32, 1: TF32 mode) with the colour-blend export (kp.row_blend [rfn][rn*dn])
+template <int G, int NP>
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_blend(const KParams kp) { point_body<G, false, NP, true>(kp); }
 
 }  // namespace pm3

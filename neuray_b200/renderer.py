@@ -42,6 +42,8 @@ base_cfg = {
     "render_depth": False,
     # each pass' visibility_nr [1,rn,rfn]: every pixel's visibility from each working view (nr_view_visibility)
     "render_visibility": False,
+    # each pass' blend_weights_nr [1,rn,rfn]: every pixel's colour-blend weight per working view (nr_render_pass_fwd_blend)
+    "render_blend_weights": False,
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
@@ -284,9 +286,11 @@ class PassLaunch(NamedTuple):
     stream: int
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32):
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False):
     """Enqueues the two kernels of the pass pp; returns its raw outputs (ray_mask as uint8) and its PassLaunch, None when
-    there are no rays.  tf32: the point kernel in TF32 mode (set_precision)."""
+    there are no rays.  tf32: the point kernel in TF32 mode (set_precision).  blend: the point kernel also exports its
+    colour-blend weights and a reduction forms blend_weights [1,rn,rfn] (nr_render_pass_fwd_blend, _tf32_blend): Σ_d
+    hit_prob · the reference's blending_weights_valid (ibrnet.py:362-366) of each view."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
@@ -305,6 +309,8 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
         "render_depth": torch.empty(1, rn, dtype=torch.float32, device=dev),
         "ray_mask_u8": torch.empty(1, rn, dtype=torch.uint8, device=dev),
     }
+    if blend:
+        out["blend_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
     rec = _lib.workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
     p = _lib.NrPassParams()
     p.coords, p.que_depth, p.que_cam = _lib.ptr(coords_c), _lib.ptr(que_depth), _lib.ptr(cam)
@@ -331,7 +337,15 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     if rn == 0:          # nothing to render: the (empty) outputs are already in place
         return out, None
     with _lib.on_device(coords):
-        if _lib.PROFILE is not None:
+        if blend:
+            if _lib.PROFILE is not None:
+                raise _lib.NeurayB200Error("the point kernel is timed alone only without render_blend_weights")
+            b = _lib.NrBlendParams()
+            b.row_blend = _lib.ptr(_lib.workspace("row_blend", pack.rfn * rn * dn, dev))
+            b.blend_weights = _lib.ptr(out["blend_weights"])
+            entry = "nr_render_pass_fwd_tf32_blend" if tf32 else "nr_render_pass_fwd_blend"
+            _lib.check(getattr(_lib.lib(), entry)(C.byref(p), C.byref(b), stream), entry)
+        elif _lib.PROFILE is not None:
             # bench.py: time the dominant kernel alone, with CUDA events on the launching stream
             e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
             e0.record()
@@ -347,7 +361,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             _lib.check(_lib.lib().nr_render_pass_fwd_tf32(C.byref(p), stream), "nr_render_pass_fwd_tf32")
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
-    _lib.count_launches(2)
+    _lib.count_launches(3 if blend else 2)
     return out, PassLaunch(p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
 
 
@@ -355,8 +369,9 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     """One fused pass.  que_depth [1,rn,dn].  `fine`: None or dict(dn=, use_all=, u=, u_stride=) to also emit the
     next pass' depths.  Returns dict with pixel_colors [1,rn,3], hit_prob [1,rn,dn], render_depth [1,rn],
     ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M], with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
-    hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises) and, with cfg
-    render_visibility, visibility [1,rn,rfn] (no gradient: requires_grad is False).
+    hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises), with cfg
+    render_visibility, visibility [1,rn,rfn] and, with cfg render_blend_weights, blend_weights [1,rn,rfn] (neither has a
+    gradient: requires_grad is False).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
@@ -373,8 +388,9 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     params = [v for _, v in pp.named]
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for v in params))
     want_dr, want_vis = owner.cfg["use_dr_prediction"], owner.cfg.get("render_visibility", False)
-    out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit or want_vis,
-                               PRECISION == "tf32" and not needs_grad)
+    want_blend = owner.cfg.get("render_blend_weights", False)
+    out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit or want_vis or want_blend,
+                               PRECISION == "tf32" and not needs_grad, want_blend)
     dr = _direct_render(owner, launch, rn, dn, coords.device) if want_dr else None
     if want_vis:
         out["visibility"] = _view_visibility(launch, out["hit_prob"], rn, rf.shape[0], coords.device)
@@ -394,7 +410,7 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
 # the optional outputs of a pass: (cfg switch, run_pass key, output key)
 _OPTIONAL_OUTPUTS = (("use_dr_prediction", "pixel_colors_dr", "pixel_colors_dr"), ("use_dr_prediction", "hit_prob_dr", "hit_prob_dr"),
                      ("use_ray_mask", "ray_mask", "ray_mask"), ("render_depth", "render_depth", "render_depth"),
-                     ("render_visibility", "visibility", "visibility_nr"))
+                     ("render_visibility", "visibility", "visibility_nr"), ("render_blend_weights", "blend_weights", "blend_weights_nr"))
 
 
 def _finish_outputs(owner, res, que_imgs_info):

@@ -6,12 +6,13 @@ render after warm-up.
                 use_nr_color_for_dr)
     tf32        black_800 and fern_high: renderer.set_precision "fp32" (3xTF32) and "tf32"
     visibility  black_800 and fern_high: cfg render_visibility off and on
+    blend       black_800 and fern_high: cfg render_blend_weights off and on
 
 Prints one JSON line: the card name, power limit and SM clocks read in the same run; per workload and arm the median
 frame time and ray-samples/s with their ranges; and the option's summary (dr_cost_ms, speedup_median and
-max_abs_diff_pixel_colors_nr_fine, visibility_cost_ms_median).  With --point-kernel, _lib.PROFILE also times the point
-kernel alone (events around each point-kernel launch).
-usage: python tools/pass_option_time.py {dr,tf32,visibility} [frames] [--point-kernel]"""
+max_abs_diff_pixel_colors_nr_fine, visibility_cost_ms_median, blend_cost_ms_median).  With --point-kernel, _lib.PROFILE
+also times the point kernel alone (events around each point-kernel launch); the blend export has no such timing.
+usage: python tools/pass_option_time.py {dr,tf32,visibility,blend} [frames] [--point-kernel]"""
 import argparse
 import json
 import os
@@ -48,12 +49,18 @@ def visibility_summary(entry, outs):
     return {"visibility_cost_ms_median": round(entry["on"]["frame_ms"]["median"] - entry["off"]["frame_ms"]["median"], 1)}
 
 
+def blend_summary(entry, outs):
+    assert finite(outs["on"]["blend_weights_nr"], outs["on"]["blend_weights_nr_fine"])
+    return {"blend_cost_ms_median": round(entry["on"]["frame_ms"]["median"] - entry["off"]["frame_ms"]["median"], 1)}
+
+
 # option -> (workloads, {arm: (cfg overrides, render precision)}, summary)
 OPTIONS = {
     "dr": (("black_800",), {"dr_off": ({}, "fp32"), "dr_sh": ({"use_dr_prediction": True}, "fp32"),
                             "dr_nr_color": ({"use_dr_prediction": True, "use_nr_color_for_dr": True}, "fp32")}, dr_summary),
     "tf32": (("black_800", "fern_high"), {"fp32": ({}, "fp32"), "tf32": ({}, "tf32")}, tf32_summary),
     "visibility": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_visibility": True}, "fp32")}, visibility_summary),
+    "blend": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_blend_weights": True}, "fp32")}, blend_summary),
 }
 
 ap = argparse.ArgumentParser(description="per-frame cost of a render-pass option")
@@ -61,6 +68,8 @@ ap.add_argument("option", choices=OPTIONS)
 ap.add_argument("frames", nargs="?", type=int, default=5)
 ap.add_argument("--point-kernel", action="store_true", help="also time the point kernel alone")
 args = ap.parse_args()
+if args.option == "blend" and args.point_kernel:
+    ap.error("the point kernel with the blend export is not timed alone")
 assert torch.cuda.is_available(), "pass_option_time.py measures on a GPU"
 dev = torch.device("cuda")
 
