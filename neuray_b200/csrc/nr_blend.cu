@@ -40,8 +40,7 @@ __global__ void __launch_bounds__(THREADS) blend_weights_kernel(const float* __r
       const int d = lane + 32 * j;
       if (d < dn) acc = fmaf(hit[j], __ldg(w + d), acc);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    acc = warp_sum(acc);
     if (lane == v) mine = acc;
   }
   if (lane < rfn) blend_weights[ray * rfn + lane] = mine;

@@ -12,6 +12,14 @@ namespace nr {
 
 void set_error(const char* fmt, ...);
 
+// Launch helpers (nr_ops.cu).  On a failed CUDA call both set an error naming `who` and return NR_E_CUDA.
+// The SM count of the current device.
+int sm_count(int* sms, const char* who);
+// The dynamic shared-memory opt-in of kernel `fn` for a launch with `bytes` of it (nothing to do at or below 48 KB).  It
+// is a per-device function attribute and is set on every launch, so that the library keeps no per-process state: a
+// process may render on any number of devices from any number of threads.
+int opt_in_smem(const void* fn, size_t bytes, const char* who);
+
 #define NR_CHECK_ARG(cond, msg)                    \
   do {                                             \
     if (!(cond)) {                                 \
@@ -185,6 +193,14 @@ __device__ __forceinline__ float softplusf_(float x) { return x > 20.f ? x : fma
 __device__ __forceinline__ float logistic_cdf(float x) {
   // 0.5 + 0.5*tanh(x) = 1/(1+exp(-2x))
   return 1.f / (1.f + __expf(-2.f * x));
+}
+
+// sum over each aligned group of L lanes (a power of two), xor butterfly L/2, ..., 1; every lane of the group gets the sum
+template <int L = 32, class T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+  for (int o = L / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
 }
 
 // read-only input: the non-coherent load path on the device

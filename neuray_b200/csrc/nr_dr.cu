@@ -43,10 +43,7 @@ extern "C" int nr_direct_render(const NrPassParams* p, const NrDrParams* d, void
   const int w_floats = (p->use_vis ? 4 : 3) * lay::DD_HEAD_STRIDE;
   const size_t smem = sizeof(float) * (w_floats + (d->use_nr_color ? 0 : size_t(dr::THREADS) * p->rfn * dr::ROW));
   static_assert(lay::DD_HEAD == 0 && lay::DD_HEAD_STRIDE % 4 == 0, "the decoder heads are staged as float4 from offset 0");
-  if (cudaFuncSetAttribute(dr::dr_point_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-    set_error("nr_direct_render: %zu bytes of shared memory", smem);
-    return NR_E_CUDA;
-  }
+  if (opt_in_smem((const void*)dr::dr_point_kernel, smem, "nr_direct_render") != NR_OK) return NR_E_CUDA;
   const long long N = (long long)p->rn * p->dn;
   cudaStream_t s = (cudaStream_t)stream;
   dr::dr_point_kernel<<<unsigned((N + dr::THREADS - 1) / dr::THREADS), dr::THREADS, smem, s>>>(*p, *d, w_floats);

@@ -1,36 +1,10 @@
 // Encoders upstream of the ray path on the GPU (SURVEY.md 8(f) row f1): kernels for the building blocks of nr_conv.cuh, the
 // stream backend of the layer graphs of nr_encoder_graph.cuh, and the C-ABI entry points (include/neuray_b200.h).
 #include "nr_encoder_graph.cuh"
+#include "nr_tc.cuh"
 
 namespace nr {
 namespace cv {
-
-__device__ __forceinline__ void cp_async16_zfill(float* dst, const float* src, bool valid) {
-  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
-  const int n = valid ? 16 : 0;                                  // src-size 0: nothing is read, the 16 bytes are zero-filled
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(d), "l"(src), "r"(n) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-
-// D (16x8, fp32) += A (16x8, tf32, row) * B (8x8, tf32, col), warp-level tensor-core MMA
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-// x = hi + lo, hi exact in tf32 (low 13 mantissa bits cleared), lo = x - hi exact in fp32
-__device__ __forceinline__ void split(float x, uint32_t& hi, uint32_t& lo) {
-  hi = __float_as_uint(x) & 0xffffe000u;
-  lo = __float_as_uint(x - __uint_as_float(hi));
-}
-
-__device__ __forceinline__ uint32_t to_tf32(float x) {      // round to nearest (the MMA itself would truncate)
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return r;
-}
 
 // FAST = one TF32 pass per product (operands rounded to TF32: ~1e-3 relative, torch's default for cuDNN convolutions);
 // otherwise the 3xTF32 split (fp32 accuracy, what the parity tests run)
@@ -59,13 +33,13 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
       int dst;
       const float* src;
       a_chunk<KC>(p, ri[j], a_row + j * A_ROWS, a_c4, kt, dst, src);
-      cp_async16_zfill(A + dst, src != nullptr ? src : p.x, src != nullptr);
+      tc::cp_async16_zfill(A + dst, src != nullptr ? src : p.x, src != nullptr);
     }
     for (int idx = tid; idx < KC * BN / 4; idx += THREADS) {
       int dst;
       const float* src;
       b_chunk<BN, KC>(p, idx, kt, dst, src);
-      cp_async16_zfill(B + dst, src, true);
+      tc::cp_async16_zfill(B + dst, src, true);
     }
   };
 
@@ -80,13 +54,13 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
 #pragma unroll
   for (int s = 0; s < STAGES - 1; ++s) {
     if (s < nk) stage(s, s);
-    cp_async_commit();
+    tc::cp_async_commit();
   }
   for (int kt = 0; kt < nk; ++kt) {
-    cp_async_wait<STAGES - 2>();      // this thread's copies of step kt have landed ...
+    tc::cp_async_wait<STAGES - 2>();  // this thread's copies of step kt have landed ...
     __syncthreads();                  // ... and everybody's; everybody is also done with the slot refilled next
     if (kt + STAGES - 1 < nk) stage(kt + STAGES - 1, (kt + STAGES - 1) % STAGES);
-    cp_async_commit();
+    tc::cp_async_commit();
     const float* A = sm + (kt % STAGES) * ST;
     const float* B = A + A_ST;
     // The tensor cores add into their fp32 accumulator with truncation (measured: 1e-7 of the running sum per MMA, always
@@ -108,8 +82,8 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
         a_frag<KC>(warp_m * (16 * MT) + 16 * i, lane, k8, off);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          if constexpr (FAST) ah[i][e] = to_tf32(A[off[e]]);
-          else split(A[off[e]], ah[i][e], al[i][e]);
+          if constexpr (FAST) ah[i][e] = tc::tf32_rna(A[off[e]]);
+          else tc::split_tf32(A[off[e]], ah[i][e], al[i][e]);
         }
       }
 #pragma unroll
@@ -118,8 +92,8 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
         b_frag<BN>(warp_n * 32 + 8 * j, lane, k8, off);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          if constexpr (FAST) bh[j][e] = to_tf32(B[off[e]]);
-          else split(B[off[e]], bh[j][e], bl[j][e]);
+          if constexpr (FAST) bh[j][e] = tc::tf32_rna(B[off[e]]);
+          else tc::split_tf32(B[off[e]], bh[j][e], bl[j][e]);
         }
       }
 #pragma unroll
@@ -127,10 +101,10 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           if constexpr (!FAST) {
-            mma_tf32(part[i][j], al[i], bh[j]);      // small terms first
-            mma_tf32(part[i][j], ah[i], bl[j]);
+            tc::mma_tf32_m16n8k8(part[i][j], al[i], bh[j]);      // small terms first
+            tc::mma_tf32_m16n8k8(part[i][j], ah[i], bl[j]);
           }
-          mma_tf32(part[i][j], ah[i], bh[j]);
+          tc::mma_tf32_m16n8k8(part[i][j], ah[i], bh[j]);
         }
     }
 #pragma unroll
@@ -140,7 +114,7 @@ __global__ void __launch_bounds__(THREADS, BN >= 128 ? 1 : 2) conv_mma_kernel(co
 #pragma unroll
         for (int e = 0; e < 4; ++e) acc[i][j][e] += part[i][j][e];
   }
-  cp_async_wait<0>();
+  tc::cp_async_wait<0>();
 
   // InstanceNorm sums: thread partials -> the 8 row lanes of a warp (shuffles) -> the CTA (shared memory) -> ONE fp64 atomic
   // per (column, sum) and CTA.  Thousands of CTAs adding to the same 2 x Cout addresses of an image serialise in L2: with one
@@ -216,11 +190,8 @@ __global__ void __launch_bounds__(256) conv7_kernel(const __grid_constant__ Conv
 #pragma unroll
   for (int c = 0; c < COUT; ++c) {
     float sv = out[c], qv = out[c] * out[c];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      sv += __shfl_xor_sync(0xffffffffu, sv, o);
-      qv += __shfl_xor_sync(0xffffffffu, qv, o);
-    }
+    sv = warp_sum(sv);
+    qv = warp_sum(qv);
     if ((threadIdx.x & 31) == 0) {
       atomicAdd(&cta_sums[2 * c], double(sv));
       atomicAdd(&cta_sums[2 * c + 1], double(qv));
@@ -387,7 +358,7 @@ __global__ void __launch_bounds__(256) pack_params_kernel(const __grid_constant_
 template <int BM, int BN, int KC, bool FAST>
 int launch_conv_f(const ConvP& p, cudaStream_t st) {
   constexpr size_t smem = size_t(stages_of(BM)) * (BM * (KC + 4) + KC * (BN + 8)) * sizeof(float);
-  cudaFuncSetAttribute(conv_mma_kernel<BM, BN, KC, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));   // per device, per launch
+  if (opt_in_smem((const void*)conv_mma_kernel<BM, BN, KC, FAST>, smem, "conv_mma_kernel") != NR_OK) return NR_E_CUDA;
   const long long M = (long long)p.N * p.Ho * p.Wo;
   conv_mma_kernel<BM, BN, KC, FAST><<<unsigned((M + BM - 1) / BM), THREADS, smem, st>>>(p);
   NR_CHECK_LAUNCH("conv_mma_kernel");
@@ -415,12 +386,12 @@ int check_conv(const ConvP& p) {
   return NR_OK;
 }
 
-int sm_count();
-
 int launch_conv(const ConvP& p, cudaStream_t st) {
   const int rc = check_conv(p);
   if (rc != NR_OK) return rc;
-  const int bm = p.bm != 0 ? p.bm : pick_bm(p.Cout, (long long)p.N * p.Ho * p.Wo, sm_count());
+  int sms = 0;
+  if (p.bm == 0 && sm_count(&sms, "conv") != NR_OK) return NR_E_CUDA;
+  const int bm = p.bm != 0 ? p.bm : pick_bm(p.Cout, (long long)p.N * p.Ho * p.Wo, sms);
   switch (p.Cout) {
     case 32:
       NR_CHECK_ARG(bm == 128 || bm == 256, "conv: 128 or 256 pixels per CTA for 32 outputs");
@@ -481,13 +452,6 @@ struct StreamOps {
     cudaMemsetAsync(ptr, 0, bytes, st);
   }
 };
-
-int sm_count() {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 132;
-}
 
 int pack_params(const enc::NetSpec& spec, const float* const* params, int n_params, float* packed, cudaStream_t st) {
   NR_CHECK_ARG(params != nullptr && packed != nullptr, "pack: null pointer");
@@ -573,8 +537,10 @@ extern "C" int nr_image_encoder_fwd(const float* packed, const float* imgs, int 
   enc::build_image_net(net);
   const long long stats = enc::image_stats_doubles(net, n, h, w);
   NR_CHECK_ARG(stats > 0, "image_encoder: image size the decoder's skip connections cannot take (ops.py:199-208)");
+  int sms;
+  if (sm_count(&sms, "image_encoder") != NR_OK) return NR_E_CUDA;
   enc::Arena ar{(char*)workspace, size_t(workspace_bytes), 0, true};
-  cv::StreamOps ops{(cudaStream_t)stream, cv::sm_count(), NR_OK, tf32x1 != 0};
+  cv::StreamOps ops{(cudaStream_t)stream, sms, NR_OK, tf32x1 != 0};
   const bool ok = enc::image_encoder_graph(ops, ar, net, packed, imgs, n, h, w, out, out_stride, out_off, stats, nullptr);
   if (ops.rc != NR_OK) return ops.rc;
   NR_CHECK_ARG(ok, "image_encoder: workspace too small (nr_image_encoder_workspace)");
@@ -590,8 +556,10 @@ extern "C" int nr_vis_encoder_fwd(const float* packed, float* feat, int n, int f
   enc::VisNet net;
   enc::build_vis_net(net);
   const long long stats = enc::vis_stats_doubles(net, n, fh, fw);
+  int sms;
+  if (sm_count(&sms, "vis_encoder") != NR_OK) return NR_E_CUDA;
   enc::Arena ar{(char*)workspace, size_t(workspace_bytes), 0, true};
-  cv::StreamOps ops{(cudaStream_t)stream, cv::sm_count(), NR_OK, tf32x1 != 0};
+  cv::StreamOps ops{(cudaStream_t)stream, sms, NR_OK, tf32x1 != 0};
   const bool ok = enc::vis_encoder_graph(ops, ar, net, packed, feat, n, fh, fw, stats, nullptr);
   if (ops.rc != NR_OK) return ops.rc;
   NR_CHECK_ARG(ok, "vis_encoder: workspace too small (nr_vis_encoder_workspace)");
@@ -602,8 +570,10 @@ extern "C" int nr_vis_encoder_fwd(const float* packed, float* feat, int n, int f
 extern "C" int nr_extract_depth(const float* depth, const float* depth_range, int n, int h, int w, float* out, void* stream) {
   if (n == 0) return NR_OK;
   NR_CHECK_ARG(depth && depth_range && out && n >= 1 && h >= 1 && w >= 1, "extract_depth");
+  int sms;
+  if (sm_count(&sms, "extract_depth") != NR_OK) return NR_E_CUDA;
   const long long hw = (long long)h * w;
-  cv::extract_depth_kernel<<<cv::grid_for((long long)n * hw, 16 * cv::sm_count()), 256, 0, (cudaStream_t)stream>>>(depth, depth_range, n, hw, out);
+  cv::extract_depth_kernel<<<cv::grid_for((long long)n * hw, 16 * sms), 256, 0, (cudaStream_t)stream>>>(depth, depth_range, n, hw, out);
   NR_CHECK_LAUNCH("extract_depth_kernel");
   return NR_OK;
 }
@@ -636,6 +606,8 @@ extern "C" int nr_depth_init_fwd(const float* packed, const float* imgs, const f
   NR_CHECK_ARG(packed && imgs && depth_norm && diff_feats && out && workspace, "depth_init: null pointer");
   NR_CHECK_ARG(n >= 1 && h >= 32 && w >= 32, "depth_init: images must be at least 32 x 32");
   NR_CHECK_ARG(out_stride >= 32 && out_stride % 4 == 0 && out_off % 4 == 0 && out_off + 32 <= out_stride, "depth_init: output channel slot");
+  int sms;
+  if (sm_count(&sms, "depth_init") != NR_OK) return NR_E_CUDA;
   enc::DepthInitNet* net = new enc::DepthInitNet;
   enc::build_depth_init_net(*net);
   const long long stats = enc::depth_init_stats_doubles(*net, n, h, w);
@@ -652,7 +624,7 @@ extern "C" int nr_depth_init_fwd(const float* packed, const float* imgs, const f
       cv::nchw_to_nhwc_kernel<<<dim3(unsigned((hw + 31) / 32), 1, n), 256, 0, st>>>(imgs, x16, n, 3, hw, 16, 0);
       cv::nchw_to_nhwc_kernel<<<dim3(unsigned((hw + 31) / 32), 1, n), 256, 0, st>>>(depth_norm, x16, n, 1, hw, 16, 3);
       cv::nchw_to_nhwc_kernel<<<dim3(unsigned((hw + 31) / 32), 1, n), 256, 0, st>>>(diff_feats, x16, n, 8, hw, 16, 4);
-      cv::StreamOps ops{st, cv::sm_count(), NR_OK, tf32x1 != 0};
+      cv::StreamOps ops{st, sms, NR_OK, tf32x1 != 0};
       ok = enc::depth_init_graph(ops, ar, *net, packed, x16, depth_norm, n, h, w, out, out_stride, out_off, stats, nullptr);
       rc = ops.rc;
     }
@@ -698,6 +670,8 @@ extern "C" int nr_cost_volume_head_fwd(int cost_volume_sn, const float* packed, 
   NR_CHECK_ARG(packed && imgs && prob && depth_norm && out && workspace, "cost_volume_head: null pointer");
   NR_CHECK_ARG(n >= 1 && h >= 32 && w >= 32 && cost_volume_sn >= 16 && cost_volume_sn % 16 == 0, "cost_volume_head: shape");
   NR_CHECK_ARG(out_stride >= 32 && out_stride % 4 == 0 && out_off % 4 == 0 && out_off + 32 <= out_stride, "cost_volume_head: output channel slot");
+  int sms;
+  if (sm_count(&sms, "cost_volume_head") != NR_OK) return NR_E_CUDA;
   enc::CostVolumeHead* net = new enc::CostVolumeHead;
   enc::build_cost_volume_head(*net, cost_volume_sn);
   const enc::ImageDims d = enc::image_dims(h, w);
@@ -712,7 +686,7 @@ extern "C" int nr_cost_volume_head_fwd(int cost_volume_sn, const float* packed, 
     if (ar.ok) {
       cudaMemsetAsync(d16, 0, size_t(n) * hw * 16 * sizeof(float), st);
       cv::nchw_to_nhwc_kernel<<<dim3(unsigned((hw + 31) / 32), 1, n), 256, 0, st>>>(depth_norm, d16, n, 1, hw, 16, 0);
-      cv::StreamOps ops{st, cv::sm_count(), NR_OK, tf32x1 != 0};
+      cv::StreamOps ops{st, sms, NR_OK, tf32x1 != 0};
       ok = enc::cost_volume_head_graph(ops, ar, *net, packed, imgs, prob, cost_volume_sn, d16, n, h, w, d.u2h, d.u2w, out, out_stride, out_off, stats, nullptr);
       rc = ops.rc;
     }
@@ -763,7 +737,9 @@ extern "C" int nr_instance_norm_act(const float* x, const double* stats, const f
   p.x = x; p.stats = stats; p.gamma = gamma; p.beta = beta; p.res = res; p.res_stats = res_stats; p.res_gamma = res_gamma; p.res_beta = res_beta;
   p.y = y; p.N = n; p.HW = hw; p.C = c; p.act = act; p.x_stride = c; p.x_off = 0; p.res_stride = c; p.res_off = 0; p.y_stride = c; p.y_off = 0;
   p.eps = 1e-5f;
-  cv::StreamOps ops{(cudaStream_t)stream, cv::sm_count(), NR_OK, 0};
+  int sms;
+  if (sm_count(&sms, "instance_norm_act") != NR_OK) return NR_E_CUDA;
+  cv::StreamOps ops{(cudaStream_t)stream, sms, NR_OK, 0};
   ops.norm(p);
   NR_CHECK_LAUNCH("norm_act_kernel");
   return NR_OK;

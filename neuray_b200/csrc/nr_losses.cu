@@ -14,20 +14,16 @@ __global__ void __launch_bounds__(64) depth_mean_kernel(const __grid_constant__ 
 // sum of (a, b) over the block's threads; result valid in thread 0
 __device__ __forceinline__ void block_sum2(double& a, double& b) {
   __shared__ double sa[32], sb[32];
-  for (int o = 16; o > 0; o >>= 1) {
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-  }
+  a = warp_sum(a);
+  b = warp_sum(b);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (lane == 0) { sa[warp] = a; sb[warp] = b; }
   __syncthreads();
   if (warp == 0) {
     a = lane < (blockDim.x >> 5) ? sa[lane] : 0.0;
     b = lane < (blockDim.x >> 5) ? sb[lane] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) {
-      a += __shfl_xor_sync(0xffffffffu, a, o);
-      b += __shfl_xor_sync(0xffffffffu, b, o);
-    }
+    a = warp_sum(a);
+    b = warp_sum(b);
   }
 }
 

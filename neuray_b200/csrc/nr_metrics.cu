@@ -38,7 +38,7 @@ struct Args {
 // sum over the block in a fixed order; the result is valid in thread 0
 template <class T>
 __device__ __forceinline__ T block_sum(T v, T* red) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   __syncthreads();
   if (lane == 0) red[warp] = v;
@@ -369,13 +369,6 @@ __device__ __forceinline__ float sum_sq(float4 v) {
   return __fadd_rn(__fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y)), __fadd_rn(__fmul_rn(v.z, v.z), __fmul_rn(v.w, v.w)));
 }
 
-template <int L>
-__device__ __forceinline__ float group_sum(float v) {      // over the L aligned lanes of a group; every lane gets the sum
-#pragma unroll
-  for (int o = L / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // One tap, steps 3-4 of LPIPS for TAP_PIX pixels of one pair (blockIdx.y): per pixel, each image's features divided by
 // (their channel norm + 1e-10), the squared difference weighted by lin and summed over the channels.  A group of L lanes
 // holds one pixel's C channels.  part[pair * stride + block] = the sum over the block's pixels, added in a fixed order.
@@ -406,7 +399,7 @@ __global__ void __launch_bounds__(THREADS) tap_kernel(const float* __restrict__ 
       s0 = __fadd_rn(s0, sum_sq(a[v]));
       s1 = __fadd_rn(s1, sum_sq(b[v]));
     }
-    const float n0 = sqrtf(group_sum<L>(s0)) + 1e-10f, n1 = sqrtf(group_sum<L>(s1)) + 1e-10f;
+    const float n0 = sqrtf(warp_sum<L>(s0)) + 1e-10f, n1 = sqrtf(warp_sum<L>(s1)) + 1e-10f;
     float t = 0.f;
 #pragma unroll
     for (int v = 0; v < V; ++v) {
@@ -414,7 +407,7 @@ __global__ void __launch_bounds__(THREADS) tap_kernel(const float* __restrict__ 
       const float dz = a[v].z / n0 - b[v].z / n1, dw = a[v].w / n0 - b[v].w / n1;
       t += wl[v].x * dx * dx + wl[v].y * dy * dy + wl[v].z * dz * dz + wl[v].w * dw * dw;
     }
-    t = group_sum<L>(t);
+    t = warp_sum<L>(t);
     if (valid && sub == 0) acc += t;
   }
   acc = mt::block_sum(acc, red);

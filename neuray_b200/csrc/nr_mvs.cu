@@ -178,9 +178,8 @@ extern "C" int nr_mvsnet_fwd(const float* packed, const NrMvsIn* a, float* prob,
   mvs::MvsNet net;
   mvs::build_mvsnet(net);
   enc::Arena ar{(char*)workspace, size_t(workspace_bytes), 0, true};
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int sms;
+  if (sm_count(&sms, "mvsnet") != NR_OK) return NR_E_CUDA;
   mvs::StreamOps ops{(cudaStream_t)stream, sms, NR_OK};
   const bool ok = mvs::mvsnet_graph(ops, ar, net, packed, packed + net.total, to_in(a), prob, depth);
   if (ops.rc != NR_OK) return ops.rc;

@@ -259,6 +259,26 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+// A failed query is not sticky: cudaGetLastError() clears it, so that the next launch check does not report it again.
+int sm_count(int* sms, const char* who) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess) return NR_OK;
+  cudaGetLastError();
+  set_error("%s: cannot query the SM count: %s", who, cudaGetErrorString(e));
+  return NR_E_CUDA;
+}
+
+int opt_in_smem(const void* fn, size_t bytes, const char* who) {
+  if (bytes <= 48 * 1024) return NR_OK;
+  const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes));
+  if (e == cudaSuccess) return NR_OK;
+  cudaGetLastError();
+  set_error("%s: cannot opt in to %zu bytes of dynamic shared memory: %s", who, bytes, cudaGetErrorString(e));
+  return NR_E_CUDA;
+}
+
 }  // namespace nr
 
 using namespace nr;
@@ -424,8 +444,7 @@ int nr_sample_fine_depth(const float* depth, const float* hit_prob, const float*
   while (warps > 1 && size_t(warps) * per_warp * 4 > 160 * 1024) warps >>= 1;
   const size_t smem = size_t(warps) * per_warp * 4;
   NR_CHECK_ARG(smem <= 200 * 1024, "sample_fine_depth shared memory");
-  if (smem > 48 * 1024)   // per-device attribute, set per launch: no per-process state (see nr_point_kernel.cu)
-    cudaFuncSetAttribute(fine_depth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (opt_in_smem((const void*)fine_depth_kernel, smem, "sample_fine_depth") != NR_OK) return NR_E_CUDA;
   const int grid = min((rn + warps - 1) / warps, 132 * 8);
   fine_depth_kernel<<<grid, warps * 32, smem, (cudaStream_t)stream>>>(depth, hit_prob, depth_range, rn, dn, fine_dn, u, u_stride,
                                                                       use_all, do_sort, sort_n, per_warp, out);

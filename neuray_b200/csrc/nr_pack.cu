@@ -42,9 +42,10 @@ __device__ __forceinline__ void put_tc(float* wt, int off, tcl::Tile t, int n, i
   if constexpr (TF32) {
     wt[pos + t.hi] = __uint_as_float(tc::tf32_rna(v));
   } else {
-    const float hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-    wt[pos + t.hi] = hi;
-    wt[pos + t.lo] = v - hi;
+    uint32_t hi, lo;
+    tc::split_tf32(v, hi, lo);
+    wt[pos + t.hi] = __uint_as_float(hi);
+    wt[pos + t.lo] = __uint_as_float(lo);
   }
 }
 // an entry of w_point / w_ray (the TF32 pack writes neither)

@@ -113,12 +113,6 @@ struct Blk {
 
 namespace pm {
 template <int G>
-__device__ __forceinline__ float bsum(float x) {
-#pragma unroll
-  for (int o = G / 2; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-  return x;
-}
-template <int G>
 __device__ __forceinline__ float bmax(float x) {
 #pragma unroll
   for (int o = G / 2; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
@@ -301,16 +295,6 @@ __device__ __forceinline__ void ld_cols(const float* __restrict__ row, int v, fl
 
 }  // namespace pkt
 
-static int device_sms() {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
-
-// The dynamic shared-memory opt-in is a per-device function attribute; it is set on every launch (a few hundred
-// nanoseconds against a kernel of milliseconds) so that the library keeps no per-process state: a process may render on
-// any number of devices from any number of threads.
 // TF32: the TF32-mode kernel (release form only), else the 3xTF32 one; BLEND: the release form with the colour-blend
 // export (kp.row_blend)
 template <int G, bool DEBUG, bool TF32, bool BLEND = false>
@@ -320,10 +304,7 @@ static int launch_pm3_inst(const pkt::KParams& kp, int grid, cudaStream_t stream
   if constexpr (BLEND) fn = pkt::pm3::point_kernel_blend<G, TF32 ? 1 : 3>;
   else if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
   else fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
-  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(pkt::pm3::SMEM_BYTES)) != cudaSuccess) {
-    nr::set_error("point kernel: cannot opt in to %zu bytes of shared memory: %s", pkt::pm3::SMEM_BYTES, cudaGetErrorString(cudaGetLastError()));
-    return NR_E_CUDA;
-  }
+  if (opt_in_smem((const void*)fn, pkt::pm3::SMEM_BYTES, "point kernel") != NR_OK) return NR_E_CUDA;
   fn<<<grid, pkt::pm3::NTHR, pkt::pm3::SMEM_BYTES, stream>>>(kp);
   NR_CHECK_LAUNCH(BLEND ? "point_kernel_blend" : TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
   return NR_OK;
@@ -335,7 +316,8 @@ static int launch_pm3(pkt::KParams kp, bool tf32, cudaStream_t stream) {
   const long long N = (long long)kp.p.rn * kp.p.dn;
   kp.P = PB;
   kp.n_tiles = int((N + PB - 1) / PB);
-  const int sms = device_sms();
+  int sms;
+  if (sm_count(&sms, "point kernel") != NR_OK) return NR_E_CUDA;
   const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
   if (kp.row_blend)
     return tf32 ? launch_pm3_inst<G, false, true, true>(kp, grid, stream) : launch_pm3_inst<G, false, false, true>(kp, grid, stream);

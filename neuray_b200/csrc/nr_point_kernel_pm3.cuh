@@ -37,7 +37,6 @@
 
 namespace pm3 {
 
-using pm::bsum;
 using pm::bmax;
 using pm::bsum_vec;
 using pm::own_col;
@@ -624,7 +623,7 @@ __device__ __forceinline__ void point_body(const KParams& kp) {
   float* const stg = smem + OFF_STG + warp * 32 * STG_ROW;
   float* const xch = smem + OFF_XCH;
   // sums / maxima over the lanes of a point
-  auto gsum = [&](float x) { if constexpr (P2) return bsum<G>(x); else return gsum_np2<G>(stg, lane, lane0, idle, x); };
+  auto gsum = [&](float x) { if constexpr (P2) return warp_sum<G>(x); else return gsum_np2<G>(stg, lane, lane0, idle, x); };
   auto gmax = [&](float x) { if constexpr (P2) return bmax<G>(x); else return gmax_np2<G>(stg, lane, lane0, idle, x); };
   auto gpool16 = [&](const float (&in)[16], float (&out)[16]) {
     if constexpr (P2) pool_rows<G, 16>(stg, lane, lane0, v, in, out); else pool_rows_np2<G, 16>(stg, lane, lane0, v, idle, in, out);

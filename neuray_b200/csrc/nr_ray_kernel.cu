@@ -22,8 +22,6 @@ struct KParams {
   int sort_n;         // power of two >= number of output fine samples (0 if no resampling)
 };
 
-__device__ __forceinline__ float warp_sum(float v) { return warp_sum_f(v); }
-
 __global__ void __launch_bounds__(512) ray_kernel(const KParams kp) {
   extern __shared__ __align__(16) float smem[];
   const NrPassParams& pp = kp.p;
@@ -260,11 +258,9 @@ int launch_ray_kernel(const NrPassParams* p, cudaStream_t stream) {
   kp.warps = warps;
   const size_t smem = size_t(shared_common + warps * kp.per_warp) * 4;
   NR_CHECK_ARG(smem <= 227 * 1024, "ray kernel shared memory");
-  if (smem > 48 * 1024)   // per-device attribute, set per launch: no per-process state
-    cudaFuncSetAttribute(rk::ray_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (opt_in_smem((const void*)rk::ray_kernel, smem, "ray_kernel") != NR_OK) return NR_E_CUDA;
+  int sms;
+  if (sm_count(&sms, "ray_kernel") != NR_OK) return NR_E_CUDA;
   int grid = (p->rn + warps - 1) / warps;
   const int cap = sms * 4;
   if (grid > cap) grid = cap;

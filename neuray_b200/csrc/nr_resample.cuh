@@ -5,12 +5,6 @@
 
 namespace nr {
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // hit: [dn] hit probabilities (shared or global); qd: [dn] depths of the current samples (global)
 // sT [dn], sCdf [dn+1], sSort [sort_n] are per-warp shared scratch.  out: [fine_dn (+dn)] global.
 // inv: resample in normalised inverse depth (inv_mode=True, the renderer's mode); otherwise directly in depth.
@@ -23,7 +17,7 @@ __device__ __forceinline__ void resample_ray(const float* hit, const float* __re
     sT[s] = inv ? (-1.f / __ldg(qd + s) - a) / (b - a) : __ldg(qd + s);
     psum += hit[s] + 1e-5f;
   }
-  psum = warp_sum_f(psum);
+  psum = warp_sum(psum);
   __syncwarp();
   if (lane == 0) {   // torch.cumsum on the CPU accumulates float inputs in double
     double acc = 0.0;

@@ -8,6 +8,7 @@
 // cuBLAS runs these shapes (M, N <= 64, K = 262 144) as sgemm_largek at ~320 us each, 26 per pass; the fp32 SIMT version of
 // this kernel took 1.8 ms per pass (LDS/FMA bound).
 #include "nr_train_math.cuh"
+#include "nr_tc.cuh"
 
 namespace nr {
 namespace tg {
@@ -26,31 +27,6 @@ struct Args {
   int first_cta[MAXD + 1];   // CTAs [first_cta[l], first_cta[l+1]) work on layer l (shares proportional to the layer's cost)
   int n_desc;
 };
-
-__device__ __forceinline__ void cp_async4(float* dst, const float* src, bool valid) {
-  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
-  const int n = valid ? 4 : 0;                                   // src-size 0: the destination is zero-filled
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(d), "l"(src), "r"(n) : "memory");
-}
-__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
-  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-
-// D (16x8, fp32) += A (16x8, tf32, row) * B (8x8, tf32, col) on the tensor cores (warp-level MMA)
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-// x = hi + lo, hi exact in tf32 (low 13 mantissa bits cleared), lo = x - hi exact in fp32
-__device__ __forceinline__ void split(float x, uint32_t& hi, uint32_t& lo) {
-  hi = __float_as_uint(x) & 0xffffe000u;
-  lo = __float_as_uint(x - __uint_as_float(hi));
-}
 
 // One CTA = (layer, contiguous range of 64-row chunks).  dW = dz * x^T is a GEMM whose contraction index is the ROW
 // (K = 262 144 at the training shape) with at most 64 x 141 outputs, so it runs as warp-level tensor-core MMAs with the
@@ -98,25 +74,25 @@ __global__ void __launch_bounds__(256) tape_gemm_kernel(const __grid_constant__ 
       for (int idx = threadIdx.x; idx < n; idx += 256) {
         const int row = idx / (KC / 4), k = (idx - row * (KC / 4)) * 4;
         const float* src = row < n_in - 1 ? xsrc + row * tr::TILE + k : zsrc + (row - (n_in - 1)) * tr::TILE + k;
-        cp_async16(buf + (row < n_in - 1 ? row : row + 1) * LDK + k, src);                // row n_in - 1 is the constant input
+        tc::cp_async16(buf + (row < n_in - 1 ? row : row + 1) * LDK + k, src);                // row n_in - 1 is the constant input
       }
     } else {                                         // the last, partial chunk: element-wise with zero fill
       const int n = (n_in - 1 + n_out) * KC;
       for (int idx = threadIdx.x; idx < n; idx += 256) {
         const int row = idx / KC, k = idx - row * KC;
         const float* src = row < n_in - 1 ? xsrc + row * tr::TILE + k : zsrc + (row - (n_in - 1)) * tr::TILE + k;
-        cp_async4(buf + (row < n_in - 1 ? row : row + 1) * LDK + k, src, k < kn);
+        tc::cp_async4_zfill(buf + (row < n_in - 1 ? row : row + 1) * LDK + k, src, k < kn);
       }
     }
   };
   for (int i = threadIdx.x; i < 2 * KC; i += 256) sm[(i / KC) * buf_floats + (n_in - 1) * LDK + (i % KC)] = 1.f;
   if (ch0 < ch_end) stage(ch0, sm);
-  cp_async_commit();
+  tc::cp_async_commit();
   for (long long ch = ch0; ch < ch_end; ++ch) {
     float* buf = sm + int((ch - ch0) & 1) * buf_floats;
     if (ch + 1 < ch_end) stage(ch + 1, sm + int((ch - ch0 + 1) & 1) * buf_floats);
-    cp_async_commit();
-    cp_async_wait<1>();
+    tc::cp_async_commit();
+    tc::cp_async_wait<1>();
     __syncthreads();
     const float* xs = buf;                       // [n_in][LDK]
     const float* zs = buf + n_in * LDK;          // [n_out][LDK]
@@ -137,11 +113,12 @@ __global__ void __launch_bounds__(256) tape_gemm_kernel(const __grid_constant__ 
         for (int ks = kpart; ks < KC / 8; ks += ksplit) {
           const int k = 8 * ks;
           uint32_t ah[4], al[4], bh[2], bl[2];
-          split(za[k], ah[0], al[0]); split(zb[k], ah[1], al[1]); split(za[k + 4], ah[2], al[2]); split(zb[k + 4], ah[3], al[3]);
-          split(xb[k], bh[0], bl[0]); split(xb[k + 4], bh[1], bl[1]);
-          mma_tf32(part, al, bh);
-          mma_tf32(part, ah, bl);
-          mma_tf32(part, ah, bh);
+          tc::split_tf32(za[k], ah[0], al[0]); tc::split_tf32(zb[k], ah[1], al[1]);
+          tc::split_tf32(za[k + 4], ah[2], al[2]); tc::split_tf32(zb[k + 4], ah[3], al[3]);
+          tc::split_tf32(xb[k], bh[0], bl[0]); tc::split_tf32(xb[k + 4], bh[1], bl[1]);
+          tc::mma_tf32_m16n8k8(part, al, bh);
+          tc::mma_tf32_m16n8k8(part, ah, bl);
+          tc::mma_tf32_m16n8k8(part, ah, bh);
         }
 #pragma unroll
         for (int e = 0; e < 4; ++e) acc[u][e] += part[e];
@@ -193,13 +170,11 @@ extern "C" int nr_tape_gemms(const NrGemmDesc* descs, int n_desc, const float* t
   a.slots[0] = tr::R_SLOTS; a.slots[1] = tr::G_SLOTS; a.slots[2] = tr::P_SLOTS; a.slots[3] = tr::GP_SLOTS;
   a.out = out;
   const size_t smem = 2 * size_t(max_rows) * tg::LDK * sizeof(float);     // two chunk buffers
-  if (smem > 48 * 1024)   // per-device attribute, set per launch: no per-process state
-    cudaFuncSetAttribute(tg::tape_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (opt_in_smem((const void*)tg::tape_gemm_kernel, smem, "tape_gemms") != NR_OK) return NR_E_CUDA;
   // CTAs per layer in proportion to its cost (bytes staged + MMAs issued per chunk), so that the 64 x 141 layers do not
   // leave a tail behind the 1 x 9 ones: ~8 CTAs per SM in total, every layer at least one
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int sms;
+  if (sm_count(&sms, "tape_gemms") != NR_OK) return NR_E_CUDA;
   double cost[tg::MAXD], total = 0.0;
   for (int i = 0; i < n_desc; ++i) {
     const NrGemmDesc& d = descs[i];

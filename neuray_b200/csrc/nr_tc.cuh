@@ -1,6 +1,8 @@
-// wgmma / TMA / mbarrier primitives for the tensor-core MLP layers (sm_90a).
+// Tensor-core and async-copy primitives of every kernel (sm_90a): wgmma and mma.sync, the TF32 operand forms (3xTF32
+// split, round to nearest), TMA bulk copies, mbarriers and cp.async.  The 3xTF32 split is also the format of the hi / lo
+// slots nr_pack_weights writes, so the packer and the kernels share one definition of it.
 //
-// Layer shape used throughout:  D[128 x N] (fp32) += A[128 x K] (tf32, smem) * B[N x K]^T (tf32, smem), issued as one
+// wgmma layer shape (point kernel, self-test):  D[128 x N] (fp32) += A[128 x K] (tf32, smem) * B[N x K]^T (tf32, smem), issued as one
 // m64nNk8 wgmma per K = 8 step for each row half (rows 0..63 and 64..127): by two warp groups, one half each (point
 // kernel), or both halves by one warp group (self-test)
 //   * A lives in a per-block shared-memory activation tile: row r = the row thread r of the warp group owns, one fp32 column
@@ -60,6 +62,22 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// ---- cp.async (global -> shared, per thread; completion by commit / wait groups) ----
+__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+// !valid: nothing is read (src-size 0) and the destination is zero-filled
+__device__ __forceinline__ void cp_async16_zfill(float* dst, const float* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async4_zfill(float* dst, const float* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 4 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+// wait until at most N of this thread's committed groups are in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+
 // named barrier among `count` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
@@ -240,7 +258,7 @@ __device__ __forceinline__ void acc_store(float* act, int dcol, int t, const flo
   acc_store_half<N>(act, dcol, t, 1, d[1]);
 }
 
-// 3xTF32 split
+// 3xTF32 split: hi = x with the low 13 mantissa bits cleared (exact in tf32), lo = x - hi (exact in fp32)
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xffffe000u;
   lo = __float_as_uint(x - __uint_as_float(hi));

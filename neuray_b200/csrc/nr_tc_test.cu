@@ -113,25 +113,26 @@ extern "C" int nr_tc_selftest(const float* A, const float* W, float* D, int n, i
   NR_CHECK_ARG(mode >= 0 && mode <= 2, "mode");
   auto run = [&](auto* fn, int k_) {
     const int smem = (2 * k_ + 64) / 32 * 4096 * 4;
-    cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (nr::opt_in_smem((const void*)fn, smem, "nr_tc_selftest") != NR_OK) return NR_E_CUDA;
     fn<<<1, 128, smem, s>>>(A, W, D);
+    NR_CHECK_LAUNCH("tc_selftest");
+    return NR_OK;
   };
   // the mode is a template argument: a runtime loop around the wgmma batch makes ptxas serialise it
   if (n == 32 && k == 32) {
-    if (mode == 0) run(nr::tc_selftest_kernel<32, 32, 0>, 32);
-    else if (mode == 1) run(nr::tc_selftest_kernel<32, 32, 1>, 32);
-    else run(nr::tc_selftest_kernel<32, 32, 2>, 32);
-  } else if (n == 64 && k == 64 && mode < 2) {
-    if (mode == 0) run(nr::tc_selftest_kernel<64, 64, 0>, 64);
-    else run(nr::tc_selftest_kernel<64, 64, 1>, 64);
-  } else if (n == 16 && k == 64) {
-    if (mode == 0) run(nr::tc_selftest_kernel<16, 64, 0>, 64);
-    else if (mode == 1) run(nr::tc_selftest_kernel<16, 64, 1>, 64);
-    else run(nr::tc_selftest_kernel<16, 64, 2>, 64);
-  } else {
-    nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d mode=%d", n, k, mode);
-    return NR_E_UNSUPPORTED;
+    if (mode == 0) return run(nr::tc_selftest_kernel<32, 32, 0>, 32);
+    if (mode == 1) return run(nr::tc_selftest_kernel<32, 32, 1>, 32);
+    return run(nr::tc_selftest_kernel<32, 32, 2>, 32);
   }
-  NR_CHECK_LAUNCH("tc_selftest");
-  return NR_OK;
+  if (n == 64 && k == 64 && mode < 2) {
+    if (mode == 0) return run(nr::tc_selftest_kernel<64, 64, 0>, 64);
+    return run(nr::tc_selftest_kernel<64, 64, 1>, 64);
+  }
+  if (n == 16 && k == 64) {
+    if (mode == 0) return run(nr::tc_selftest_kernel<16, 64, 0>, 64);
+    if (mode == 1) return run(nr::tc_selftest_kernel<16, 64, 1>, 64);
+    return run(nr::tc_selftest_kernel<16, 64, 2>, 64);
+  }
+  nr::set_error("nr_tc_selftest: unsupported shape n=%d k=%d mode=%d", n, k, mode);
+  return NR_E_UNSUPPORTED;
 }

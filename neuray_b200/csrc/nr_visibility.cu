@@ -49,14 +49,10 @@ extern "C" int nr_view_visibility(const NrPassParams* p, const NrVisParams* q, v
   const int w_floats = (p->use_vis ? 4 : 3) * lay::DD_HEAD_STRIDE;
   const size_t smem = sizeof(float) * (w_floats + size_t(vis::THREADS) * p->rfn);
   static_assert(lay::DD_HEAD == 0 && lay::DD_HEAD_STRIDE % 4 == 0, "the decoder heads are staged as float4 from offset 0");
-  if (cudaFuncSetAttribute(vis::view_visibility_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-    set_error("nr_view_visibility: %zu bytes of shared memory", smem);
-    return NR_E_CUDA;
-  }
-  int dev = 0, sms = 0, per_sm = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vis::view_visibility_kernel, vis::THREADS, smem) != cudaSuccess ||
-      per_sm == 0) {
+  if (opt_in_smem((const void*)vis::view_visibility_kernel, smem, "nr_view_visibility") != NR_OK) return NR_E_CUDA;
+  int sms = 0, per_sm = 0;
+  if (sm_count(&sms, "nr_view_visibility") != NR_OK) return NR_E_CUDA;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vis::view_visibility_kernel, vis::THREADS, smem) != cudaSuccess || per_sm == 0) {
     set_error("nr_view_visibility: no occupancy for %zu bytes of shared memory", smem);
     return NR_E_CUDA;
   }
