@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define NR_ABI_VERSION 12
+#define NR_ABI_VERSION 13
 
 #define NR_OK 0
 #define NR_E_INVALID (-1)   /* bad argument (null pointer, unsupported shape) */
@@ -212,6 +212,29 @@ typedef struct NrBlendParams {
 } NrBlendParams;
 int nr_render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);
 int nr_render_pass_fwd_tf32_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);   /* TF32 mode */
+
+/* Per-view weights of each rendered pixel inside the aggregation net (cfg render_agg_weights): nr_render_pass_fwd (or
+ * _tf32) with the point kernel also exporting each (view, point) row's two pooling weights and its blend weight, then one
+ * reduction kernel per output, the one of nr_render_pass_fwd_blend:
+ *   neuray_weights[r, v]   = Σ_d hit_prob[r, d] · weight0[v, r, d]
+ *   geometry_weights[r, v] = Σ_d hit_prob[r, d] · weight[v, r, d]
+ *   blend_weights[r, v]    as in nr_render_pass_fwd_blend (skipped when blend_weights is NULL)
+ * weight0 is the reference's NeuRay weight of the same pass (ibrnet.py:334-337: sigmoid(neuray_fc) · mask / (Σ_v mask +
+ * 1e-8), the weight of the first pooled mean/variance), weight its geometry weight (ibrnet.py:349-350: vis / (Σ_v vis +
+ * 1e-8) with vis = vis_fc2(x · vis) · mask, the weight of the pooling in front of geometry_fc); hit_prob is the pass'
+ * compositing weight (p->hit_prob is required).  Σ_v weight = Σ_v vis / (Σ_v vis + 1e-8), weight0 <= mask / (Σ_v mask +
+ * 1e-8), and a point that no view sees has 0 in both.  Views in view_params order; unnormalised, like render_depth.  The
+ * sums run in an order fixed by dn alone, so a ray's result does not depend on the chunk or launch that renders it.  Every
+ * other output equals the one of nr_render_pass_fwd (or _blend) bit for bit.  Four or five kernels, no host
+ * synchronisation. */
+typedef struct NrAggParams {
+  float* rows;               /* workspace [3, rfn, rn*dn]: blend weight, weight0, weight */
+  float* neuray_weights;     /* [rn,rfn] */
+  float* geometry_weights;   /* [rn,rfn] */
+  float* blend_weights;      /* [rn,rfn], or NULL */
+} NrAggParams;
+int nr_render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, void* stream);
+int nr_render_pass_fwd_tf32_agg(const NrPassParams* p, const NrAggParams* a, void* stream);   /* TF32 mode */
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);

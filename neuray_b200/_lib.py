@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # NEURAY_B200_LIB: development switch to load another in-tree build of the same library (A/B runs of kernel variants)
 LIB_PATH = os.environ.get("NEURAY_B200_LIB") or os.path.join(_HERE, "libneuray_b200.so")
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 NR_POINT_REC = 20
 NR_MAX_VIEWS = 32
 NR_MAX_SAMPLES = 256
@@ -56,6 +56,10 @@ class NrBlendParams(C.Structure):
     _fields_ = [("row_blend", C.c_void_p), ("blend_weights", C.c_void_p)]
 
 
+class NrAggParams(C.Structure):
+    _fields_ = [("rows", C.c_void_p), ("neuray_weights", C.c_void_p), ("geometry_weights", C.c_void_p), ("blend_weights", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -89,6 +93,8 @@ SIGNATURES = {
     "nr_view_visibility": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrVisParams), _vp]),
     "nr_render_pass_fwd_blend": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrBlendParams), _vp]),
     "nr_render_pass_fwd_tf32_blend": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrBlendParams), _vp]),
+    "nr_render_pass_fwd_agg": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrAggParams), _vp]),
+    "nr_render_pass_fwd_tf32_agg": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrAggParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),

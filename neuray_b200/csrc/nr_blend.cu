@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(THREADS) blend_weights_kernel(const float* __r
 }  // namespace blend
 
 // The reduction of nr_render_pass_fwd_blend / _tf32_blend, enqueued behind the pass that filled b->row_blend and
-// p->hit_prob.
+// p->hit_prob.  nr_render_pass_fwd_agg / _tf32_agg run it once per output, each on its [rfn][rn*dn] row of the export.
 int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, cudaStream_t stream) {
   if (p->rn == 0) return NR_OK;
   const long long blocks = ((long long)p->rn + blend::THREADS / 32 - 1) / (blend::THREADS / 32);

@@ -230,14 +230,14 @@ __global__ void fine_depth_kernel(const float* __restrict__ depth, const float* 
 }  // namespace ops
 
 // implemented in nr_point_kernel.cu / nr_ray_kernel.cu / nr_blend.cu
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* row_blend, bool tf32, cudaStream_t stream);
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* rows, int exports, bool tf32, cudaStream_t stream);
 int launch_ray_kernel(const NrPassParams* p, cudaStream_t stream);
 int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, cudaStream_t stream);
 
-// One render pass: the point kernel (3xTF32 or TF32 mode; row_blend: optional export of its colour-blend weights), then
-// the ray kernel.  Every nr_render_pass_fwd* entry point is this sequence.
-static int render_pass_fwd(const NrPassParams* p, float* row_blend, bool tf32, cudaStream_t stream) {
-  const int rc = launch_point_kernel(p, nullptr, nullptr, row_blend, tf32, stream);
+// One render pass: the point kernel (3xTF32 or TF32 mode; rows, exports: its optional per-row exports, EXPORT_BLEND
+// and EXPORT_AGG), then the ray kernel.  Every nr_render_pass_fwd* entry point is this sequence.
+static int render_pass_fwd(const NrPassParams* p, float* rows, int exports, bool tf32, cudaStream_t stream) {
+  const int rc = launch_point_kernel(p, nullptr, nullptr, rows, exports, tf32, stream);
   if (rc != NR_OK) return rc;
   return launch_ray_kernel(p, stream);
 }
@@ -246,9 +246,28 @@ static int render_pass_fwd(const NrPassParams* p, float* row_blend, bool tf32, c
 static int render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr && b != nullptr, "params");
   if (p->rn > 0) NR_CHECK_ARG(b->row_blend && b->blend_weights && p->hit_prob, "null blend workspace, blend_weights or hit_prob");
-  const int rc = render_pass_fwd(p, b->row_blend, tf32, stream);
+  const int rc = render_pass_fwd(p, b->row_blend, EXPORT_BLEND, tf32, stream);
   if (rc != NR_OK) return rc;
   return launch_blend_weights(p, b, stream);
+}
+
+// The pass with the blend and pooling-weight exports on, then the same reduction once per requested output, each on its
+// row of the workspace: the blend weight (unless a->blend_weights is NULL), w0 (neuray_weights) and w2 (geometry_weights).
+static int render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, bool tf32, cudaStream_t stream) {
+  NR_CHECK_ARG(p != nullptr && a != nullptr, "params");
+  if (p->rn > 0)
+    NR_CHECK_ARG(a->rows && a->neuray_weights && a->geometry_weights && p->hit_prob,
+                 "null agg workspace, neuray_weights, geometry_weights or hit_prob");
+  int rc = render_pass_fwd(p, a->rows, EXPORT_BLEND | EXPORT_AGG, tf32, stream);
+  if (rc != NR_OK) return rc;
+  const size_t plane = size_t(p->rfn) * p->rn * p->dn;          // one [rfn][rn*dn] row of the workspace
+  const NrBlendParams outs[3] = {{a->rows, a->blend_weights}, {a->rows + plane, a->neuray_weights},
+                                 {a->rows + 2 * plane, a->geometry_weights}};
+  for (const NrBlendParams& b : outs) {
+    if (b.blend_weights == nullptr) continue;                    // only the blend weight is optional
+    if ((rc = launch_blend_weights(p, &b, stream)) != NR_OK) return rc;
+  }
+  return NR_OK;
 }
 
 static thread_local char g_err[512] = "";
@@ -332,24 +351,30 @@ int nr_pack_feature_maps(const float* ray_feats, const float* img_feats, const f
   return NR_OK;
 }
 
-int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, false, (cudaStream_t)stream); }
-int nr_point_kernel_tf32(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, true, (cudaStream_t)stream); }
+int nr_point_kernel(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, 0, false, (cudaStream_t)stream); }
+int nr_point_kernel_tf32(const NrPassParams* p, void* stream) { return launch_point_kernel(p, nullptr, nullptr, nullptr, 0, true, (cudaStream_t)stream); }
 int nr_point_kernel_debug(const NrPassParams* p, float* dbg, void* stream) {
   NR_CHECK_ARG(dbg != nullptr, "dbg");
-  return launch_point_kernel(p, dbg, nullptr, nullptr, false, (cudaStream_t)stream);
+  return launch_point_kernel(p, dbg, nullptr, nullptr, 0, false, (cudaStream_t)stream);
 }
 int nr_point_kernel_timing(const NrPassParams* p, long long* timing, void* stream) {
   NR_CHECK_ARG(timing != nullptr && p != nullptr && p->w_tc != nullptr, "timing buffer / tensor-core weights required");
-  return launch_point_kernel(p, nullptr, timing, nullptr, false, (cudaStream_t)stream);
+  return launch_point_kernel(p, nullptr, timing, nullptr, 0, false, (cudaStream_t)stream);
 }
 int nr_ray_kernel(const NrPassParams* p, void* stream) { return launch_ray_kernel(p, (cudaStream_t)stream); }
-int nr_render_pass_fwd(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, false, (cudaStream_t)stream); }
-int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, true, (cudaStream_t)stream); }
+int nr_render_pass_fwd(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, 0, false, (cudaStream_t)stream); }
+int nr_render_pass_fwd_tf32(const NrPassParams* p, void* stream) { return render_pass_fwd(p, nullptr, 0, true, (cudaStream_t)stream); }
 int nr_render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, void* stream) {
   return render_pass_fwd_blend(p, b, false, (cudaStream_t)stream);
 }
 int nr_render_pass_fwd_tf32_blend(const NrPassParams* p, const NrBlendParams* b, void* stream) {
   return render_pass_fwd_blend(p, b, true, (cudaStream_t)stream);
+}
+int nr_render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, void* stream) {
+  return render_pass_fwd_agg(p, a, false, (cudaStream_t)stream);
+}
+int nr_render_pass_fwd_tf32_agg(const NrPassParams* p, const NrAggParams* a, void* stream) {
+  return render_pass_fwd_agg(p, a, true, (cudaStream_t)stream);
 }
 
 int nr_sample_depth(const float* depth_range, int rn, int dn, const float* jitter, float* depth, float* dists, void* stream) {

@@ -43,7 +43,7 @@ struct KParams {
   NrPassParams p;
   float* dbg;
   long long* timing;   // optional: clock64() at phase boundaries, CTA 0, thread 0 of each compute warp group: [tile][2][32]
-  float* row_blend;    // optional: each valid (view, point) row's colour-blend weight, [rfn][rn*dn] (warp group 1, end of tile)
+  float* rows;         // optional per-row exports, [k][rfn][rn*dn]: the colour-blend weight, then (EXPORT_AGG) w0, w2
   int P, n_tiles, n_heads;
 };
 
@@ -295,23 +295,25 @@ __device__ __forceinline__ void ld_cols(const float* __restrict__ row, int v, fl
 
 }  // namespace pkt
 
-// TF32: the TF32-mode kernel (release form only), else the 3xTF32 one; BLEND: the release form with the colour-blend
-// export (kp.row_blend)
-template <int G, bool DEBUG, bool TF32, bool BLEND = false>
+// TF32: the TF32-mode kernel (release form only), else the 3xTF32 one; EXPORTS: the release form with that export set
+// (kp.rows): EXPORT_BLEND alone or with EXPORT_AGG
+template <int G, bool DEBUG, bool TF32, int EXPORTS = 0>
 static int launch_pm3_inst(const pkt::KParams& kp, int grid, cudaStream_t stream) {
-  static_assert(!(TF32 && DEBUG) && !(BLEND && DEBUG), "the TF32 mode and the blend export have no debug form");
+  static_assert(!(TF32 && DEBUG) && !(EXPORTS && DEBUG), "the TF32 mode and the exports have no debug form");
+  static_assert(EXPORTS == 0 || EXPORTS == EXPORT_BLEND || EXPORTS == (EXPORT_BLEND | EXPORT_AGG), "export sets");
   void (*fn)(const pkt::KParams);
-  if constexpr (BLEND) fn = pkt::pm3::point_kernel_blend<G, TF32 ? 1 : 3>;
+  if constexpr (EXPORTS == (EXPORT_BLEND | EXPORT_AGG)) fn = pkt::pm3::point_kernel_agg<G, TF32 ? 1 : 3>;
+  else if constexpr (EXPORTS == EXPORT_BLEND) fn = pkt::pm3::point_kernel_blend<G, TF32 ? 1 : 3>;
   else if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
   else fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
   if (opt_in_smem((const void*)fn, pkt::pm3::SMEM_BYTES, "point kernel") != NR_OK) return NR_E_CUDA;
   fn<<<grid, pkt::pm3::NTHR, pkt::pm3::SMEM_BYTES, stream>>>(kp);
-  NR_CHECK_LAUNCH(BLEND ? "point_kernel_blend" : TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
+  NR_CHECK_LAUNCH(EXPORTS & EXPORT_AGG ? "point_kernel_agg" : EXPORTS ? "point_kernel_blend" : TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
   return NR_OK;
 }
 
 template <int G>
-static int launch_pm3(pkt::KParams kp, bool tf32, cudaStream_t stream) {
+static int launch_pm3(pkt::KParams kp, int exports, bool tf32, cudaStream_t stream) {
   constexpr int PB = 4 * (32 / G);       // points per 128-row block: 32 / G per warp (G not a power of two leaves 32 % G lanes idle)
   const long long N = (long long)kp.p.rn * kp.p.dn;
   kp.P = PB;
@@ -319,19 +321,24 @@ static int launch_pm3(pkt::KParams kp, bool tf32, cudaStream_t stream) {
   int sms;
   if (sm_count(&sms, "point kernel") != NR_OK) return NR_E_CUDA;
   const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
-  if (kp.row_blend)
-    return tf32 ? launch_pm3_inst<G, false, true, true>(kp, grid, stream) : launch_pm3_inst<G, false, false, true>(kp, grid, stream);
+  constexpr int AGG = EXPORT_BLEND | EXPORT_AGG;
+  if (exports & EXPORT_AGG)
+    return tf32 ? launch_pm3_inst<G, false, true, AGG>(kp, grid, stream) : launch_pm3_inst<G, false, false, AGG>(kp, grid, stream);
+  if (exports)
+    return tf32 ? launch_pm3_inst<G, false, true, EXPORT_BLEND>(kp, grid, stream) : launch_pm3_inst<G, false, false, EXPORT_BLEND>(kp, grid, stream);
   if (tf32) return launch_pm3_inst<G, false, true>(kp, grid, stream);
   return (kp.dbg || kp.timing) ? launch_pm3_inst<G, true, false>(kp, grid, stream) : launch_pm3_inst<G, false, false>(kp, grid, stream);
 }
 
 // `timing`: optional clock64() stamps at the phase boundaries (nr_point_kernel_timing), passed per call.  tf32: the TF32
-// mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.  row_blend: optional
-// [rfn][rn*dn] export of the colour-blend weights (nr_render_pass_fwd_blend / _tf32_blend), in either mode.
-int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* row_blend, bool tf32, cudaStream_t stream) {
+// mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.  exports: 0, EXPORT_BLEND
+// ([rfn][rn*dn] colour-blend weights in rows: nr_render_pass_fwd_blend / _tf32_blend) or EXPORT_BLEND | EXPORT_AGG
+// ([3][rfn][rn*dn]: those, then w0 and w2: nr_render_pass_fwd_agg / _tf32_agg), in either mode.
+int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* rows, int exports, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr, "params");
   NR_CHECK_ARG(!tf32 || (dbg == nullptr && timing == nullptr), "the TF32 point kernel has no debug tap or phase stamps");
-  NR_CHECK_ARG(!row_blend || (dbg == nullptr && timing == nullptr), "the blend export has no debug tap or phase stamps");
+  NR_CHECK_ARG(exports == 0 || exports == EXPORT_BLEND || exports == (EXPORT_BLEND | EXPORT_AGG), "export set");
+  NR_CHECK_ARG(!exports || (dbg == nullptr && timing == nullptr), "the exports have no debug tap or phase stamps");
   NR_CHECK_ARG(p->coords && p->que_depth && p->que_cam && p->feat && p->rgb && p->view_params && p->w_point && p->point_rec,
                "null device pointer");
   NR_CHECK_ARG(p->w_tc != nullptr, "w_tc (tensor-core weight buffer, nr_pack_weights) is required");
@@ -346,16 +353,16 @@ int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, fl
   kp.p = *p;
   kp.dbg = dbg;
   kp.timing = timing;
-  kp.row_blend = row_blend;
+  kp.rows = rows;
   kp.n_heads = p->use_vis ? 4 : 3;
   // lanes per point: the smallest group size that holds the views and wastes the fewest of a warp's 32 lanes
-  if (p->rfn <= 4) return launch_pm3<4>(kp, tf32, stream);
-  if (p->rfn == 5) return launch_pm3<5>(kp, tf32, stream);      // 6 points per warp (30 lanes) instead of 4 groups of 8
-  if (p->rfn == 6) return launch_pm3<6>(kp, tf32, stream);      // 5 points per warp
-  if (p->rfn <= 8) return launch_pm3<8>(kp, tf32, stream);
-  if (p->rfn <= 10) return launch_pm3<10>(kp, tf32, stream);    // 3 points per warp instead of 2 groups of 16 (cfg4: 10 views)
-  if (p->rfn <= 16) return launch_pm3<16>(kp, tf32, stream);
-  return launch_pm3<32>(kp, tf32, stream);
+  if (p->rfn <= 4) return launch_pm3<4>(kp, exports, tf32, stream);
+  if (p->rfn == 5) return launch_pm3<5>(kp, exports, tf32, stream);      // 6 points per warp (30 lanes) instead of 4 groups of 8
+  if (p->rfn == 6) return launch_pm3<6>(kp, exports, tf32, stream);      // 5 points per warp
+  if (p->rfn <= 8) return launch_pm3<8>(kp, exports, tf32, stream);
+  if (p->rfn <= 10) return launch_pm3<10>(kp, exports, tf32, stream);    // 3 points per warp instead of 2 groups of 16 (cfg4: 10 views)
+  if (p->rfn <= 16) return launch_pm3<16>(kp, exports, tf32, stream);
+  return launch_pm3<32>(kp, exports, tf32, stream);
 }
 
 }  // namespace nr

@@ -520,11 +520,15 @@ __device__ __forceinline__ void ld_row(const Blk& b, int col, float* v) {
   }
 }
 
-// The kernel body, NP passes per tensor-core product (point_kernel_pm3: 3, point_kernel_tf32: 1).  BLEND: warp group 1
-// also stores each valid row's colour-blend weight into kp.row_blend (point_kernel_blend); a compile-time switch, so that
-// the kernels without the export are the same code as before it existed.
-template <int G, bool DEBUG, int NP, bool BLEND = false>
+// The kernel body, NP passes per tensor-core product (point_kernel_pm3: 3, point_kernel_tf32: 1).  EXPORTS: the per-row
+// weights it also stores into kp.rows, a compile-time set so that the kernels without an export are the same code as
+// before it existed.  EXPORT_BLEND: warp group 1 stores each valid row's colour-blend weight into kp.rows[0]
+// (point_kernel_blend).  EXPORT_AGG: warp group 1 also stores the row's pooling weights, the NeuRay weight w0 into
+// kp.rows[1] and the geometry weight w2 into kp.rows[2] (point_kernel_agg, which carries EXPORT_BLEND as well); all at
+// the end of the tile.
+template <int G, bool DEBUG, int NP, int EXPORTS = 0>
 __device__ __forceinline__ void point_body(const KParams& kp) {
+  constexpr bool BLEND = (EXPORTS & EXPORT_BLEND) != 0, AGG = (EXPORTS & EXPORT_AGG) != 0;
   extern __shared__ __align__(1024) float smem[];
   constexpr bool P2 = (G & (G - 1)) == 0;      // power-of-two lane groups reduce with butterflies, the others through shared memory
   constexpr int PPW = 32 / G;                   // points per warp (G = 10: 3, two lanes idle)
@@ -1188,7 +1192,15 @@ __device__ __forceinline__ void point_body(const KParams& kp) {
       }
       // the blend weight of this (view, point) row (nr_render_pass_fwd_blend): the reference's blending_weights_valid
       if constexpr (BLEND) {
-        if (row_ok) kp.row_blend[size_t(v) * N + n] = e / acc[0];
+        if (row_ok) kp.rows[size_t(v) * N + n] = e / acc[0];
+      }
+      // the pooling weights of this row (nr_render_pass_fwd_agg): the reference's weight0 (ibrnet.py:334-337) and its
+      // weight from vis (ibrnet.py:349-350).  Both warp groups hold them; stored here, off the pooling rounds' barriers.
+      if constexpr (AGG) {
+        if (row_ok) {
+          kp.rows[size_t(rfn + v) * N + n] = w0;
+          kp.rows[size_t(2 * rfn + v) * N + n] = w2;
+        }
       }
     }
     PM_TICK(15)
@@ -1202,8 +1214,11 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_pm3(const KParams kp) { 
 // rna(W) in the hi slots (nr_pack_weights_tf32)
 template <int G>
 __global__ void __launch_bounds__(NTHR, 1) point_kernel_tf32(const KParams kp) { point_body<G, false, 1>(kp); }
-// Either release form (NP = 3: 3xTF32, 1: TF32 mode) with the colour-blend export (kp.row_blend [rfn][rn*dn])
+// Either release form (NP = 3: 3xTF32, 1: TF32 mode) with the colour-blend export (kp.rows [rfn][rn*dn])
 template <int G, int NP>
-__global__ void __launch_bounds__(NTHR, 1) point_kernel_blend(const KParams kp) { point_body<G, false, NP, true>(kp); }
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_blend(const KParams kp) { point_body<G, false, NP, EXPORT_BLEND>(kp); }
+// Either release form with the colour-blend and the pooling-weight exports (kp.rows [3][rfn][rn*dn]: blend, w0, w2)
+template <int G, int NP>
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_agg(const KParams kp) { point_body<G, false, NP, EXPORT_BLEND | EXPORT_AGG>(kp); }
 
 }  // namespace pm3

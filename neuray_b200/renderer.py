@@ -44,6 +44,9 @@ base_cfg = {
     "render_visibility": False,
     # each pass' blend_weights_nr [1,rn,rfn]: every pixel's colour-blend weight per working view (nr_render_pass_fwd_blend)
     "render_blend_weights": False,
+    # each pass' neuray_weights_nr and geometry_weights_nr [1,rn,rfn]: every pixel's weight per working view in the
+    # aggregation net's two view poolings, weight0 and the vis weight (nr_render_pass_fwd_agg)
+    "render_agg_weights": False,
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
@@ -286,11 +289,14 @@ class PassLaunch(NamedTuple):
     stream: int
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False):
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False, agg=False):
     """Enqueues the two kernels of the pass pp; returns its raw outputs (ray_mask as uint8) and its PassLaunch, None when
     there are no rays.  tf32: the point kernel in TF32 mode (set_precision).  blend: the point kernel also exports its
     colour-blend weights and a reduction forms blend_weights [1,rn,rfn] (nr_render_pass_fwd_blend, _tf32_blend): Σ_d
-    hit_prob · the reference's blending_weights_valid (ibrnet.py:362-366) of each view."""
+    hit_prob · the reference's blending_weights_valid (ibrnet.py:362-366) of each view.  agg: the point kernel also
+    exports its two pooling weights and reductions form neuray_weights and geometry_weights [1,rn,rfn]
+    (nr_render_pass_fwd_agg, _tf32_agg): Σ_d hit_prob · the reference's weight0 (ibrnet.py:334-337) and weight
+    (ibrnet.py:349-350) of each view; with blend as well, the same launch forms blend_weights."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
@@ -311,6 +317,9 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     }
     if blend:
         out["blend_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
+    if agg:
+        out["neuray_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
+        out["geometry_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
     rec = _lib.workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
     p = _lib.NrPassParams()
     p.coords, p.que_depth, p.que_cam = _lib.ptr(coords_c), _lib.ptr(que_depth), _lib.ptr(cam)
@@ -337,7 +346,16 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     if rn == 0:          # nothing to render: the (empty) outputs are already in place
         return out, None
     with _lib.on_device(coords):
-        if blend:
+        if agg:
+            if _lib.PROFILE is not None:
+                raise _lib.NeurayB200Error("the point kernel is timed alone only without render_agg_weights")
+            a = _lib.NrAggParams()
+            a.rows = _lib.ptr(_lib.workspace("row_agg", 3 * pack.rfn * rn * dn, dev))
+            a.neuray_weights, a.geometry_weights = _lib.ptr(out["neuray_weights"]), _lib.ptr(out["geometry_weights"])
+            a.blend_weights = _lib.ptr(out.get("blend_weights"))
+            entry = "nr_render_pass_fwd_tf32_agg" if tf32 else "nr_render_pass_fwd_agg"
+            _lib.check(getattr(_lib.lib(), entry)(C.byref(p), C.byref(a), stream), entry)
+        elif blend:
             if _lib.PROFILE is not None:
                 raise _lib.NeurayB200Error("the point kernel is timed alone only without render_blend_weights")
             b = _lib.NrBlendParams()
@@ -361,7 +379,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             _lib.check(_lib.lib().nr_render_pass_fwd_tf32(C.byref(p), stream), "nr_render_pass_fwd_tf32")
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
-    _lib.count_launches(3 if blend else 2)
+    _lib.count_launches(2 + (2 if agg else 0) + (1 if blend else 0))
     return out, PassLaunch(p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
 
 
@@ -370,8 +388,9 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     next pass' depths.  Returns dict with pixel_colors [1,rn,3], hit_prob [1,rn,dn], render_depth [1,rn],
     ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M], with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
     hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises), with cfg
-    render_visibility, visibility [1,rn,rfn] and, with cfg render_blend_weights, blend_weights [1,rn,rfn] (neither has a
-    gradient: requires_grad is False).
+    render_visibility, visibility [1,rn,rfn], with cfg render_blend_weights, blend_weights [1,rn,rfn] and, with cfg
+    render_agg_weights, neuray_weights and geometry_weights [1,rn,rfn] (none of these has a gradient: requires_grad is
+    False).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
@@ -388,9 +407,10 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     params = [v for _, v in pp.named]
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for v in params))
     want_dr, want_vis = owner.cfg["use_dr_prediction"], owner.cfg.get("render_visibility", False)
-    want_blend = owner.cfg.get("render_blend_weights", False)
-    out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit or want_vis or want_blend,
-                               PRECISION == "tf32" and not needs_grad, want_blend)
+    want_blend, want_agg = owner.cfg.get("render_blend_weights", False), owner.cfg.get("render_agg_weights", False)
+    out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine,
+                               want_hit or want_vis or want_blend or want_agg, PRECISION == "tf32" and not needs_grad,
+                               want_blend, want_agg)
     dr = _direct_render(owner, launch, rn, dn, coords.device) if want_dr else None
     if want_vis:
         out["visibility"] = _view_visibility(launch, out["hit_prob"], rn, rf.shape[0], coords.device)
@@ -410,7 +430,9 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
 # the optional outputs of a pass: (cfg switch, run_pass key, output key)
 _OPTIONAL_OUTPUTS = (("use_dr_prediction", "pixel_colors_dr", "pixel_colors_dr"), ("use_dr_prediction", "hit_prob_dr", "hit_prob_dr"),
                      ("use_ray_mask", "ray_mask", "ray_mask"), ("render_depth", "render_depth", "render_depth"),
-                     ("render_visibility", "visibility", "visibility_nr"), ("render_blend_weights", "blend_weights", "blend_weights_nr"))
+                     ("render_visibility", "visibility", "visibility_nr"), ("render_blend_weights", "blend_weights", "blend_weights_nr"),
+                     ("render_agg_weights", "neuray_weights", "neuray_weights_nr"),
+                     ("render_agg_weights", "geometry_weights", "geometry_weights_nr"))
 
 
 def _finish_outputs(owner, res, que_imgs_info):
