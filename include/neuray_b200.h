@@ -236,6 +236,33 @@ typedef struct NrAggParams {
 int nr_render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, void* stream);
 int nr_render_pass_fwd_tf32_agg(const NrPassParams* p, const NrAggParams* a, void* stream);   /* TF32 mode */
 
+/* Where each working view puts the surface along each rendered pixel's ray (cfg render_view_depth): nr_render_pass_fwd
+ * (or _tf32) with the point kernel also exporting each (view, point) row's masked hit probability, next to the blend and
+ * pooling weights of nr_render_pass_fwd_agg, then one reduction kernel per output, the one of nr_render_pass_fwd_blend:
+ *   view_hit[r, v]   = Σ_d hit_v[r, d]
+ *   view_depth[r, v] = Σ_d hit_v[r, d] · que_depth[r, d]
+ *   blend_weights, neuray_weights, geometry_weights   as in nr_render_pass_fwd_agg (each skipped when NULL)
+ * hit_v is the reference's masked prj_dict['hit_prob'] of the same pass (renderer.py:75-82: compute_prob(is_ref=True) of
+ * the pass' dist decoder, times the projection mask).  Both sums are unnormalised, like render_depth: view_depth / view_hit
+ * is view v's expected surface depth along the ray, comparable with render_depth / Σ_d hit_prob.  Σ_d hit_v is not bounded
+ * by 1: each bin is centred on the sample's inverse depth in view v's range but is as wide as the query's interval, and the
+ * last interval is 1e6, so the last sample carries all of the view's mass beyond it (a view whose surface lies past far
+ * reads as far).  A view that sees none of a ray's samples has exactly 0 in both.  Views in view_params order.  The sums
+ * run in an order fixed by dn alone, so a ray's result does not depend on the chunk or launch that renders it.  Every
+ * other output equals the one of nr_render_pass_fwd (or _blend, _agg) bit for bit.  p->hit_prob is required only with the
+ * blend or agg outputs.  Four to seven kernels, no host synchronisation.  This struct and the two entry points were added
+ * within NR_ABI_VERSION 13: nothing existing changed, so a host built against the earlier version-13 header still works. */
+typedef struct NrViewParams {
+  float* rows;               /* workspace [4, rfn, rn*dn]: blend weight, weight0, weight, hit */
+  float* view_hit;           /* [rn,rfn] */
+  float* view_depth;         /* [rn,rfn] */
+  float* blend_weights;      /* [rn,rfn], or NULL */
+  float* neuray_weights;     /* [rn,rfn], or NULL (together with geometry_weights) */
+  float* geometry_weights;   /* [rn,rfn], or NULL (together with neuray_weights) */
+} NrViewParams;
+int nr_render_pass_fwd_view(const NrPassParams* p, const NrViewParams* w, void* stream);
+int nr_render_pass_fwd_tf32_view(const NrPassParams* p, const NrViewParams* w, void* stream);   /* TF32 mode */
+
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);
 int nr_point_kernel_tf32(const NrPassParams* p, void* stream);   /* TF32 mode, as in nr_render_pass_fwd_tf32 */

@@ -60,6 +60,11 @@ class NrAggParams(C.Structure):
     _fields_ = [("rows", C.c_void_p), ("neuray_weights", C.c_void_p), ("geometry_weights", C.c_void_p), ("blend_weights", C.c_void_p)]
 
 
+class NrViewParams(C.Structure):
+    _fields_ = [("rows", C.c_void_p), ("view_hit", C.c_void_p), ("view_depth", C.c_void_p), ("blend_weights", C.c_void_p),
+                ("neuray_weights", C.c_void_p), ("geometry_weights", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -95,6 +100,8 @@ SIGNATURES = {
     "nr_render_pass_fwd_tf32_blend": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrBlendParams), _vp]),
     "nr_render_pass_fwd_agg": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrAggParams), _vp]),
     "nr_render_pass_fwd_tf32_agg": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrAggParams), _vp]),
+    "nr_render_pass_fwd_view": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrViewParams), _vp]),
+    "nr_render_pass_fwd_tf32_view": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrViewParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),

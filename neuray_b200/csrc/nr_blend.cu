@@ -10,6 +10,9 @@
 //                         lanes.  The order depends on dn alone and no atomics are used, so a ray's weights are the same
 //                         whichever chunk, shard or CTA renders it.  Lane v keeps view v's sum; the ray's rfn values
 //                         leave in one store.
+//
+// nr_render_pass_fwd_view runs the same kernel on the exported hit rows with the query depths as the per-sample weight
+// (view_depth) and, in its UNIT form, with a weight of 1 (view_hit: the per-sample weight is not read).
 #include "../../include/neuray_b200.h"
 #include "nr_common.cuh"
 
@@ -19,6 +22,8 @@ namespace blend {
 constexpr int THREADS = 256;
 constexpr int PER_LANE = NR_MAX_SAMPLES / 32;     // a ray's samples held by one lane
 
+// UNIT: every sample weighs 1 and hit_prob is not read
+template <bool UNIT>
 __global__ void __launch_bounds__(THREADS) blend_weights_kernel(const float* __restrict__ hit_prob, const float* __restrict__ row_blend,
                                                                  float* __restrict__ blend_weights, int rn, int dn, int rfn) {
   const int lane = threadIdx.x & 31;
@@ -29,7 +34,7 @@ __global__ void __launch_bounds__(THREADS) blend_weights_kernel(const float* __r
 #pragma unroll
   for (int j = 0; j < PER_LANE; ++j) {
     const int d = lane + 32 * j;
-    hit[j] = d < dn ? __ldg(hit_prob + ray * dn + d) : 0.f;
+    hit[j] = d < dn ? (UNIT ? 1.f : __ldg(hit_prob + ray * dn + d)) : 0.f;
   }
   float mine = 0.f;
   for (int v = 0; v < rfn; ++v) {
@@ -49,12 +54,18 @@ __global__ void __launch_bounds__(THREADS) blend_weights_kernel(const float* __r
 }  // namespace blend
 
 // The reduction of nr_render_pass_fwd_blend / _tf32_blend, enqueued behind the pass that filled b->row_blend and
-// p->hit_prob.  nr_render_pass_fwd_agg / _tf32_agg run it once per output, each on its [rfn][rn*dn] row of the export.
-int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, cudaStream_t stream) {
+// p->hit_prob.  nr_render_pass_fwd_agg / _tf32_agg and _view / _tf32_view run it once per output, each on its
+// [rfn][rn*dn] row of the export.  weight: the per-sample weight [rn, dn] (p->hit_prob, or p->que_depth for
+// view_depth), NULL for a weight of 1 (view_hit).
+int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, const float* weight, cudaStream_t stream) {
   if (p->rn == 0) return NR_OK;
   const long long blocks = ((long long)p->rn + blend::THREADS / 32 - 1) / (blend::THREADS / 32);
-  blend::blend_weights_kernel<<<unsigned(blocks), blend::THREADS, 0, stream>>>(p->hit_prob, b->row_blend, b->blend_weights, p->rn, p->dn,
-                                                                               p->rfn);
+  if (weight != nullptr)
+    blend::blend_weights_kernel<false><<<unsigned(blocks), blend::THREADS, 0, stream>>>(weight, b->row_blend, b->blend_weights, p->rn,
+                                                                                        p->dn, p->rfn);
+  else
+    blend::blend_weights_kernel<true><<<unsigned(blocks), blend::THREADS, 0, stream>>>(nullptr, b->row_blend, b->blend_weights, p->rn,
+                                                                                       p->dn, p->rfn);
   NR_CHECK_LAUNCH("blend_weights");
   return NR_OK;
 }

@@ -22,8 +22,9 @@ int opt_in_smem(const void* fn, size_t bytes, const char* who);
 
 // The point kernel's optional per-(view, point) exports (launch_point_kernel's `exports`, point_body's EXPORTS), stored
 // into a [k][rfn][rn*dn] workspace: EXPORT_BLEND the colour-blend weight (row 0), EXPORT_AGG the aggregation net's
-// pooling weights w0 and w2 (rows 1 and 2; only together with EXPORT_BLEND).
-constexpr int EXPORT_BLEND = 1, EXPORT_AGG = 2;
+// pooling weights w0 and w2 (rows 1 and 2; only together with EXPORT_BLEND), EXPORT_VIEW the dist decoder's masked hit
+// probability (row 3; only together with both).  The sets nest, so one request is served by the smallest that covers it.
+constexpr int EXPORT_BLEND = 1, EXPORT_AGG = 2, EXPORT_VIEW = 4;
 
 #define NR_CHECK_ARG(cond, msg)                    \
   do {                                             \

@@ -232,10 +232,10 @@ __global__ void fine_depth_kernel(const float* __restrict__ depth, const float* 
 // implemented in nr_point_kernel.cu / nr_ray_kernel.cu / nr_blend.cu
 int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* rows, int exports, bool tf32, cudaStream_t stream);
 int launch_ray_kernel(const NrPassParams* p, cudaStream_t stream);
-int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, cudaStream_t stream);
+int launch_blend_weights(const NrPassParams* p, const NrBlendParams* b, const float* weight, cudaStream_t stream);
 
 // One render pass: the point kernel (3xTF32 or TF32 mode; rows, exports: its optional per-row exports, EXPORT_BLEND
-// and EXPORT_AGG), then the ray kernel.  Every nr_render_pass_fwd* entry point is this sequence.
+// and EXPORT_AGG, EXPORT_VIEW), then the ray kernel.  Every nr_render_pass_fwd* entry point is this sequence.
 static int render_pass_fwd(const NrPassParams* p, float* rows, int exports, bool tf32, cudaStream_t stream) {
   const int rc = launch_point_kernel(p, nullptr, nullptr, rows, exports, tf32, stream);
   if (rc != NR_OK) return rc;
@@ -248,7 +248,7 @@ static int render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, 
   if (p->rn > 0) NR_CHECK_ARG(b->row_blend && b->blend_weights && p->hit_prob, "null blend workspace, blend_weights or hit_prob");
   const int rc = render_pass_fwd(p, b->row_blend, EXPORT_BLEND, tf32, stream);
   if (rc != NR_OK) return rc;
-  return launch_blend_weights(p, b, stream);
+  return launch_blend_weights(p, b, p->hit_prob, stream);
 }
 
 // The pass with the blend and pooling-weight exports on, then the same reduction once per requested output, each on its
@@ -265,7 +265,32 @@ static int render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, bool
                                  {a->rows + 2 * plane, a->geometry_weights}};
   for (const NrBlendParams& b : outs) {
     if (b.blend_weights == nullptr) continue;                    // only the blend weight is optional
-    if ((rc = launch_blend_weights(p, &b, stream)) != NR_OK) return rc;
+    if ((rc = launch_blend_weights(p, &b, p->hit_prob, stream)) != NR_OK) return rc;
+  }
+  return NR_OK;
+}
+
+// The pass with all three exports on (the smallest export set that holds the hit row), then the same reduction once per
+// requested output: Σ_d hit (weight 1) and Σ_d hit · que_depth on the hit row, and whichever of the blend weight and the
+// pooling weights w0, w2 were asked for (weighted by p->hit_prob, as in render_pass_fwd_agg).
+static int render_pass_fwd_view(const NrPassParams* p, const NrViewParams* w, bool tf32, cudaStream_t stream) {
+  NR_CHECK_ARG(p != nullptr && w != nullptr, "params");
+  NR_CHECK_ARG((w->neuray_weights == nullptr) == (w->geometry_weights == nullptr),
+               "neuray_weights and geometry_weights are either both set or both NULL");
+  if (p->rn > 0) {
+    NR_CHECK_ARG(w->rows && w->view_hit && w->view_depth, "null view workspace, view_hit or view_depth");
+    NR_CHECK_ARG(p->hit_prob || (!w->blend_weights && !w->neuray_weights), "hit_prob is required with blend or agg outputs");
+  }
+  int rc = render_pass_fwd(p, w->rows, EXPORT_BLEND | EXPORT_AGG | EXPORT_VIEW, tf32, stream);
+  if (rc != NR_OK) return rc;
+  const size_t plane = size_t(p->rfn) * p->rn * p->dn;          // one [rfn][rn*dn] row of the workspace
+  const NrBlendParams outs[5] = {{w->rows + 3 * plane, w->view_hit}, {w->rows + 3 * plane, w->view_depth},
+                                 {w->rows, w->blend_weights}, {w->rows + plane, w->neuray_weights},
+                                 {w->rows + 2 * plane, w->geometry_weights}};
+  const float* const weight[5] = {nullptr, p->que_depth, p->hit_prob, p->hit_prob, p->hit_prob};   // nullptr: 1
+  for (int i = 0; i < 5; ++i) {
+    if (outs[i].blend_weights == nullptr) continue;              // an optional output that was not requested
+    if ((rc = launch_blend_weights(p, &outs[i], weight[i], stream)) != NR_OK) return rc;
   }
   return NR_OK;
 }
@@ -375,6 +400,12 @@ int nr_render_pass_fwd_agg(const NrPassParams* p, const NrAggParams* a, void* st
 }
 int nr_render_pass_fwd_tf32_agg(const NrPassParams* p, const NrAggParams* a, void* stream) {
   return render_pass_fwd_agg(p, a, true, (cudaStream_t)stream);
+}
+int nr_render_pass_fwd_view(const NrPassParams* p, const NrViewParams* w, void* stream) {
+  return render_pass_fwd_view(p, w, false, (cudaStream_t)stream);
+}
+int nr_render_pass_fwd_tf32_view(const NrPassParams* p, const NrViewParams* w, void* stream) {
+  return render_pass_fwd_view(p, w, true, (cudaStream_t)stream);
 }
 
 int nr_sample_depth(const float* depth_range, int rn, int dn, const float* jitter, float* depth, float* dists, void* stream) {

@@ -43,7 +43,8 @@ struct KParams {
   NrPassParams p;
   float* dbg;
   long long* timing;   // optional: clock64() at phase boundaries, CTA 0, thread 0 of each compute warp group: [tile][2][32]
-  float* rows;         // optional per-row exports, [k][rfn][rn*dn]: the colour-blend weight, then (EXPORT_AGG) w0, w2
+  float* rows;         // optional per-row exports, [k][rfn][rn*dn]: the colour-blend weight, then (EXPORT_AGG) w0, w2,
+                       // then (EXPORT_VIEW) hit
   int P, n_tiles, n_heads;
 };
 
@@ -296,19 +297,26 @@ __device__ __forceinline__ void ld_cols(const float* __restrict__ row, int v, fl
 }  // namespace pkt
 
 // TF32: the TF32-mode kernel (release form only), else the 3xTF32 one; EXPORTS: the release form with that export set
-// (kp.rows): EXPORT_BLEND alone or with EXPORT_AGG
+// (kp.rows): EXPORT_BLEND alone, with EXPORT_AGG, or with EXPORT_AGG and EXPORT_VIEW
 template <int G, bool DEBUG, bool TF32, int EXPORTS = 0>
 static int launch_pm3_inst(const pkt::KParams& kp, int grid, cudaStream_t stream) {
   static_assert(!(TF32 && DEBUG) && !(EXPORTS && DEBUG), "the TF32 mode and the exports have no debug form");
-  static_assert(EXPORTS == 0 || EXPORTS == EXPORT_BLEND || EXPORTS == (EXPORT_BLEND | EXPORT_AGG), "export sets");
+  static_assert(EXPORTS == 0 || EXPORTS == EXPORT_BLEND || EXPORTS == (EXPORT_BLEND | EXPORT_AGG) ||
+                    EXPORTS == (EXPORT_BLEND | EXPORT_AGG | EXPORT_VIEW),
+                "export sets");
   void (*fn)(const pkt::KParams);
-  if constexpr (EXPORTS == (EXPORT_BLEND | EXPORT_AGG)) fn = pkt::pm3::point_kernel_agg<G, TF32 ? 1 : 3>;
+  if constexpr (EXPORTS & EXPORT_VIEW) fn = pkt::pm3::point_kernel_view<G, TF32 ? 1 : 3>;
+  else if constexpr (EXPORTS == (EXPORT_BLEND | EXPORT_AGG)) fn = pkt::pm3::point_kernel_agg<G, TF32 ? 1 : 3>;
   else if constexpr (EXPORTS == EXPORT_BLEND) fn = pkt::pm3::point_kernel_blend<G, TF32 ? 1 : 3>;
   else if constexpr (TF32) fn = pkt::pm3::point_kernel_tf32<G>;
   else fn = pkt::pm3::point_kernel_pm3<G, DEBUG>;
   if (opt_in_smem((const void*)fn, pkt::pm3::SMEM_BYTES, "point kernel") != NR_OK) return NR_E_CUDA;
   fn<<<grid, pkt::pm3::NTHR, pkt::pm3::SMEM_BYTES, stream>>>(kp);
-  NR_CHECK_LAUNCH(EXPORTS & EXPORT_AGG ? "point_kernel_agg" : EXPORTS ? "point_kernel_blend" : TF32 ? "point_kernel_tf32" : "point_kernel_pm3");
+  NR_CHECK_LAUNCH(EXPORTS & EXPORT_VIEW  ? "point_kernel_view"
+                  : EXPORTS & EXPORT_AGG ? "point_kernel_agg"
+                  : EXPORTS              ? "point_kernel_blend"
+                  : TF32                 ? "point_kernel_tf32"
+                                         : "point_kernel_pm3");
   return NR_OK;
 }
 
@@ -321,7 +329,9 @@ static int launch_pm3(pkt::KParams kp, int exports, bool tf32, cudaStream_t stre
   int sms;
   if (sm_count(&sms, "point kernel") != NR_OK) return NR_E_CUDA;
   const int grid = kp.n_tiles < sms ? kp.n_tiles : sms;
-  constexpr int AGG = EXPORT_BLEND | EXPORT_AGG;
+  constexpr int AGG = EXPORT_BLEND | EXPORT_AGG, VIEW = EXPORT_BLEND | EXPORT_AGG | EXPORT_VIEW;
+  if (exports & EXPORT_VIEW)
+    return tf32 ? launch_pm3_inst<G, false, true, VIEW>(kp, grid, stream) : launch_pm3_inst<G, false, false, VIEW>(kp, grid, stream);
   if (exports & EXPORT_AGG)
     return tf32 ? launch_pm3_inst<G, false, true, AGG>(kp, grid, stream) : launch_pm3_inst<G, false, false, AGG>(kp, grid, stream);
   if (exports)
@@ -333,11 +343,14 @@ static int launch_pm3(pkt::KParams kp, int exports, bool tf32, cudaStream_t stre
 // `timing`: optional clock64() stamps at the phase boundaries (nr_point_kernel_timing), passed per call.  tf32: the TF32
 // mode (p->w_tc from nr_pack_weights_tf32), which has neither the debug tap nor the stamps.  exports: 0, EXPORT_BLEND
 // ([rfn][rn*dn] colour-blend weights in rows: nr_render_pass_fwd_blend / _tf32_blend) or EXPORT_BLEND | EXPORT_AGG
-// ([3][rfn][rn*dn]: those, then w0 and w2: nr_render_pass_fwd_agg / _tf32_agg), in either mode.
+// ([3][rfn][rn*dn]: those, then w0 and w2: nr_render_pass_fwd_agg / _tf32_agg) or all three with EXPORT_VIEW
+// ([4][rfn][rn*dn]: those, then the masked hit probability: nr_render_pass_fwd_view / _tf32_view), in either mode.
 int launch_point_kernel(const NrPassParams* p, float* dbg, long long* timing, float* rows, int exports, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr, "params");
   NR_CHECK_ARG(!tf32 || (dbg == nullptr && timing == nullptr), "the TF32 point kernel has no debug tap or phase stamps");
-  NR_CHECK_ARG(exports == 0 || exports == EXPORT_BLEND || exports == (EXPORT_BLEND | EXPORT_AGG), "export set");
+  NR_CHECK_ARG(exports == 0 || exports == EXPORT_BLEND || exports == (EXPORT_BLEND | EXPORT_AGG) ||
+                   exports == (EXPORT_BLEND | EXPORT_AGG | EXPORT_VIEW),
+               "export set");
   NR_CHECK_ARG(!exports || (dbg == nullptr && timing == nullptr), "the exports have no debug tap or phase stamps");
   NR_CHECK_ARG(p->coords && p->que_depth && p->que_cam && p->feat && p->rgb && p->view_params && p->w_point && p->point_rec,
                "null device pointer");

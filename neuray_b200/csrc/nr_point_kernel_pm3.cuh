@@ -525,10 +525,11 @@ __device__ __forceinline__ void ld_row(const Blk& b, int col, float* v) {
 // before it existed.  EXPORT_BLEND: warp group 1 stores each valid row's colour-blend weight into kp.rows[0]
 // (point_kernel_blend).  EXPORT_AGG: warp group 1 also stores the row's pooling weights, the NeuRay weight w0 into
 // kp.rows[1] and the geometry weight w2 into kp.rows[2] (point_kernel_agg, which carries EXPORT_BLEND as well); all at
-// the end of the tile.
+// the end of the tile.  EXPORT_VIEW: the front's fragment lanes also store each valid row's masked hit probability into
+// kp.rows[3] where they form it (point_kernel_view, which carries EXPORT_BLEND and EXPORT_AGG as well).
 template <int G, bool DEBUG, int NP, int EXPORTS = 0>
 __device__ __forceinline__ void point_body(const KParams& kp) {
-  constexpr bool BLEND = (EXPORTS & EXPORT_BLEND) != 0, AGG = (EXPORTS & EXPORT_AGG) != 0;
+  constexpr bool BLEND = (EXPORTS & EXPORT_BLEND) != 0, AGG = (EXPORTS & EXPORT_AGG) != 0, VIEW = (EXPORTS & EXPORT_VIEW) != 0;
   extern __shared__ __align__(1024) float smem[];
   constexpr bool P2 = (G & (G - 1)) == 0;      // power-of-two lane groups reduce with butterflies, the others through shared memory
   constexpr int PPW = 32 / G;                   // points per warp (G = 10: 3, two lanes idle)
@@ -845,6 +846,14 @@ __device__ __forceinline__ void point_body(const KParams& kp) {
           if ((P2 ? rn_ < N : (rn_ < N && g < PPW)) && rv < rfn) {
             float* __restrict__ o = kp.dbg + (size_t(rv) * N + rn_) * 76;
             o[2] = hit; o[3] = visib;
+          }
+        }
+        // the masked hit probability of row rr (nr_render_pass_fwd_view): the reference's prj_dict['hit_prob']
+        // (renderer.py:75-82); the even lane of the pair stores it, once per valid (view, point) row
+        if constexpr (VIEW) {
+          if ((q & 1) == 0) {
+            const int rn_ = n - pl + (P2 ? rr / G : (rr >> 5) * PPW + g);
+            if ((P2 ? rn_ < N : (rn_ < N && g < PPW)) && rv < rfn) kp.rows[size_t(3 * rfn + rv) * N + rn_] = hit;
           }
         }
         hv01 = q & 1 ? (visib - 0.5f) * 2.f : (hit - 0.5f) * 2.f;
@@ -1220,5 +1229,10 @@ __global__ void __launch_bounds__(NTHR, 1) point_kernel_blend(const KParams kp) 
 // Either release form with the colour-blend and the pooling-weight exports (kp.rows [3][rfn][rn*dn]: blend, w0, w2)
 template <int G, int NP>
 __global__ void __launch_bounds__(NTHR, 1) point_kernel_agg(const KParams kp) { point_body<G, false, NP, EXPORT_BLEND | EXPORT_AGG>(kp); }
+// Either release form with those exports and the masked hit probability (kp.rows [4][rfn][rn*dn]: blend, w0, w2, hit)
+template <int G, int NP>
+__global__ void __launch_bounds__(NTHR, 1) point_kernel_view(const KParams kp) {
+  point_body<G, false, NP, EXPORT_BLEND | EXPORT_AGG | EXPORT_VIEW>(kp);
+}
 
 }  // namespace pm3

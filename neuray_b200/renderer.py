@@ -47,6 +47,10 @@ base_cfg = {
     # each pass' neuray_weights_nr and geometry_weights_nr [1,rn,rfn]: every pixel's weight per working view in the
     # aggregation net's two view poolings, weight0 and the vis weight (nr_render_pass_fwd_agg)
     "render_agg_weights": False,
+    # each pass' view_hit_nr and view_depth_nr [1,rn,rfn]: Σ_d of every working view's masked hit probability along the
+    # pixel's ray, alone and times the sample depth; view_depth_nr / view_hit_nr is where the view puts the surface
+    # (nr_render_pass_fwd_view)
+    "render_view_depth": False,
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
@@ -289,14 +293,17 @@ class PassLaunch(NamedTuple):
     stream: int
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False, agg=False):
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False, agg=False, view=False):
     """Enqueues the two kernels of the pass pp; returns its raw outputs (ray_mask as uint8) and its PassLaunch, None when
     there are no rays.  tf32: the point kernel in TF32 mode (set_precision).  blend: the point kernel also exports its
     colour-blend weights and a reduction forms blend_weights [1,rn,rfn] (nr_render_pass_fwd_blend, _tf32_blend): Σ_d
     hit_prob · the reference's blending_weights_valid (ibrnet.py:362-366) of each view.  agg: the point kernel also
     exports its two pooling weights and reductions form neuray_weights and geometry_weights [1,rn,rfn]
     (nr_render_pass_fwd_agg, _tf32_agg): Σ_d hit_prob · the reference's weight0 (ibrnet.py:334-337) and weight
-    (ibrnet.py:349-350) of each view; with blend as well, the same launch forms blend_weights."""
+    (ibrnet.py:349-350) of each view; with blend as well, the same launch forms blend_weights.  view: the point kernel
+    also exports each view's masked hit probability hit_v (the reference's prj_dict['hit_prob'], renderer.py:75-82) and
+    reductions form view_hit = Σ_d hit_v and view_depth = Σ_d hit_v · que_depth [1,rn,rfn] (nr_render_pass_fwd_view,
+    _tf32_view); the same launch forms whichever of the blend and agg outputs are asked for."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
@@ -320,6 +327,9 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     if agg:
         out["neuray_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
         out["geometry_weights"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
+    if view:
+        out["view_hit"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
+        out["view_depth"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
     rec = _lib.workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
     p = _lib.NrPassParams()
     p.coords, p.que_depth, p.que_cam = _lib.ptr(coords_c), _lib.ptr(que_depth), _lib.ptr(cam)
@@ -346,7 +356,17 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     if rn == 0:          # nothing to render: the (empty) outputs are already in place
         return out, None
     with _lib.on_device(coords):
-        if agg:
+        if view:
+            if _lib.PROFILE is not None:
+                raise _lib.NeurayB200Error("the point kernel is timed alone only without render_view_depth")
+            w = _lib.NrViewParams()
+            w.rows = _lib.ptr(_lib.workspace("row_view", 4 * pack.rfn * rn * dn, dev))
+            w.view_hit, w.view_depth = _lib.ptr(out["view_hit"]), _lib.ptr(out["view_depth"])
+            w.blend_weights = _lib.ptr(out.get("blend_weights"))
+            w.neuray_weights, w.geometry_weights = _lib.ptr(out.get("neuray_weights")), _lib.ptr(out.get("geometry_weights"))
+            entry = "nr_render_pass_fwd_tf32_view" if tf32 else "nr_render_pass_fwd_view"
+            _lib.check(getattr(_lib.lib(), entry)(C.byref(p), C.byref(w), stream), entry)
+        elif agg:
             if _lib.PROFILE is not None:
                 raise _lib.NeurayB200Error("the point kernel is timed alone only without render_agg_weights")
             a = _lib.NrAggParams()
@@ -379,7 +399,7 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             _lib.check(_lib.lib().nr_render_pass_fwd_tf32(C.byref(p), stream), "nr_render_pass_fwd_tf32")
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
-    _lib.count_launches(2 + (2 if agg else 0) + (1 if blend else 0))
+    _lib.count_launches(2 + (2 if view else 0) + (2 if agg else 0) + (1 if blend else 0))
     return out, PassLaunch(p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
 
 
@@ -389,8 +409,8 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M], with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
     hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises), with cfg
     render_visibility, visibility [1,rn,rfn], with cfg render_blend_weights, blend_weights [1,rn,rfn] and, with cfg
-    render_agg_weights, neuray_weights and geometry_weights [1,rn,rfn] (none of these has a gradient: requires_grad is
-    False).
+    render_agg_weights, neuray_weights and geometry_weights [1,rn,rfn] and, with cfg render_view_depth, view_hit and
+    view_depth [1,rn,rfn] (none of these has a gradient: requires_grad is False).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
@@ -408,9 +428,10 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for v in params))
     want_dr, want_vis = owner.cfg["use_dr_prediction"], owner.cfg.get("render_visibility", False)
     want_blend, want_agg = owner.cfg.get("render_blend_weights", False), owner.cfg.get("render_agg_weights", False)
+    want_view = owner.cfg.get("render_view_depth", False)
     out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine,
                                want_hit or want_vis or want_blend or want_agg, PRECISION == "tf32" and not needs_grad,
-                               want_blend, want_agg)
+                               want_blend, want_agg, want_view)
     dr = _direct_render(owner, launch, rn, dn, coords.device) if want_dr else None
     if want_vis:
         out["visibility"] = _view_visibility(launch, out["hit_prob"], rn, rf.shape[0], coords.device)
@@ -432,7 +453,8 @@ _OPTIONAL_OUTPUTS = (("use_dr_prediction", "pixel_colors_dr", "pixel_colors_dr")
                      ("use_ray_mask", "ray_mask", "ray_mask"), ("render_depth", "render_depth", "render_depth"),
                      ("render_visibility", "visibility", "visibility_nr"), ("render_blend_weights", "blend_weights", "blend_weights_nr"),
                      ("render_agg_weights", "neuray_weights", "neuray_weights_nr"),
-                     ("render_agg_weights", "geometry_weights", "geometry_weights_nr"))
+                     ("render_agg_weights", "geometry_weights", "geometry_weights_nr"),
+                     ("render_view_depth", "view_hit", "view_hit_nr"), ("render_view_depth", "view_depth", "view_depth_nr"))
 
 
 def _finish_outputs(owner, res, que_imgs_info):

@@ -8,13 +8,15 @@ render after warm-up.
     visibility  black_800 and fern_high: cfg render_visibility off and on
     blend       black_800 and fern_high: cfg render_blend_weights off and on
     agg         black_800 and fern_high: cfg render_agg_weights off, on, and on together with render_blend_weights
+    view        black_800 and fern_high: cfg render_view_depth off, on, and on together with render_agg_weights and
+                render_blend_weights
 
 Prints one JSON line: the card name, power limit and SM clocks read in the same run; per workload and arm the median
 frame time and ray-samples/s with their ranges; and the option's summary (dr_cost_ms, speedup_median and
 max_abs_diff_pixel_colors_nr_fine, visibility_cost_ms_median, blend_cost_ms_median, agg_cost_ms_median with
-agg_blend_cost_ms_median).  With --point-kernel, _lib.PROFILE also times the point kernel alone (events around each
-point-kernel launch); the blend and agg exports have no such timing.
-usage: python tools/pass_option_time.py {dr,tf32,visibility,blend,agg} [frames] [--point-kernel]"""
+agg_blend_cost_ms_median, view_cost_ms_median with view_agg_blend_cost_ms_median).  With --point-kernel, _lib.PROFILE also
+times the point kernel alone (events around each point-kernel launch); the blend, agg and view exports have no such timing.
+usage: python tools/pass_option_time.py {dr,tf32,visibility,blend,agg,view} [frames] [--point-kernel]"""
 import argparse
 import json
 import os
@@ -64,6 +66,14 @@ def agg_summary(entry, outs):
             "agg_blend_cost_ms_median": round(entry["on_blend"]["frame_ms"]["median"] - off, 1)}
 
 
+def view_summary(entry, outs):
+    for arm in ("on", "on_agg_blend"):
+        assert finite(*(outs[arm][k + sfx] for k in ("view_hit_nr", "view_depth_nr") for sfx in ("", "_fine")))
+    off = entry["off"]["frame_ms"]["median"]
+    return {"view_cost_ms_median": round(entry["on"]["frame_ms"]["median"] - off, 1),
+            "view_agg_blend_cost_ms_median": round(entry["on_agg_blend"]["frame_ms"]["median"] - off, 1)}
+
+
 # option -> (workloads, {arm: (cfg overrides, render precision)}, summary)
 OPTIONS = {
     "dr": (("black_800",), {"dr_off": ({}, "fp32"), "dr_sh": ({"use_dr_prediction": True}, "fp32"),
@@ -73,6 +83,9 @@ OPTIONS = {
     "blend": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_blend_weights": True}, "fp32")}, blend_summary),
     "agg": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_agg_weights": True}, "fp32"),
                                          "on_blend": ({"render_agg_weights": True, "render_blend_weights": True}, "fp32")}, agg_summary),
+    "view": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_view_depth": True}, "fp32"),
+                                          "on_agg_blend": ({"render_view_depth": True, "render_agg_weights": True,
+                                                            "render_blend_weights": True}, "fp32")}, view_summary),
 }
 
 ap = argparse.ArgumentParser(description="per-frame cost of a render-pass option")
@@ -80,7 +93,7 @@ ap.add_argument("option", choices=OPTIONS)
 ap.add_argument("frames", nargs="?", type=int, default=5)
 ap.add_argument("--point-kernel", action="store_true", help="also time the point kernel alone")
 args = ap.parse_args()
-if args.option in ("blend", "agg") and args.point_kernel:
+if args.option in ("blend", "agg", "view") and args.point_kernel:
     ap.error(f"the point kernel with the {args.option} export is not timed alone")
 assert torch.cuda.is_available(), "pass_option_time.py measures on a GPU"
 dev = torch.device("cuda")
