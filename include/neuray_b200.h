@@ -205,10 +205,11 @@ int nr_view_visibility(const NrPassParams* p, const NrVisParams* v, void* stream
  * compositing weight (hit_prob_nr, so p->hit_prob is required).  Views in view_params order; unnormalised, like
  * render_depth: Σ_v blend_weights[r, v] = Σ_d hit_prob[r, d].  Each ray's sum runs in an order fixed by dn alone, so a ray's
  * result does not depend on the chunk or launch that renders it.  Every other output equals the one of the twin without
- * _blend bit for bit.  Three kernels, no host synchronisation. */
+ * _blend bit for bit.  Three kernels, no host synchronisation.  blend_weights may be NULL (accepted within NR_ABI_VERSION
+ * 13): the pass still fills row_blend, for nr_view_colors, and the reduction is skipped (two kernels). */
 typedef struct NrBlendParams {
   float* row_blend;          /* workspace [rfn, rn*dn] */
-  float* blend_weights;      /* [rn,rfn] */
+  float* blend_weights;      /* [rn,rfn], or NULL */
 } NrBlendParams;
 int nr_render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);
 int nr_render_pass_fwd_tf32_blend(const NrPassParams* p, const NrBlendParams* b, void* stream);   /* TF32 mode */
@@ -262,6 +263,25 @@ typedef struct NrViewParams {
 } NrViewParams;
 int nr_render_pass_fwd_view(const NrPassParams* p, const NrViewParams* w, void* stream);
 int nr_render_pass_fwd_tf32_view(const NrPassParams* p, const NrViewParams* w, void* stream);   /* TF32 mode */
+
+/* What colour each working view puts into each rendered pixel (cfg render_view_colors): one reduction kernel, enqueued
+ * after nr_render_pass_fwd_blend, _agg or _view (or their _tf32 twins) of the same NrPassParams, on plane 0 of that
+ * call's workspace (the blend row; blend_weights may be NULL) and the pass' hit_prob:
+ *   view_colors[r, v, c] = Σ_d hit_prob[r, d] · w[v, r, d] · rgb_v[r, d, c]
+ * w is the reference's blending_weights_valid (ibrnet.py:362-366) and rgb_v its masked prj_dict['rgb'] (render_ops.py:
+ * 132-139: the view's image at the sample's projection, 0 where the projection mask is 0), the colour the aggregation net
+ * blends: rgb_out = Σ_v rgb_in · blending_weights_valid (ibrnet.py:366-367).  So Σ_v view_colors[r, v] = pixel_colors[r]
+ * up to fp32 rounding, and a view that sees none of a ray's samples has exactly 0.  Views in view_params order;
+ * unnormalised (view_colors / blend_weights is the colour the view showed, averaged over the surface).  Each ray's sums
+ * run in an order fixed by dn alone, with no atomics, so a ray's result does not depend on the chunk or launch that
+ * renders it.  One kernel, no host synchronisation, no workspace of its own.  This struct and the entry point were added
+ * within NR_ABI_VERSION 13: nothing existing changed, so a host built against the earlier version-13 header still works. */
+typedef struct NrColorParams {
+  const float* row_blend;    /* [rfn, rn*dn]: plane 0 of the workspace of the pass' _blend, _agg or _view call */
+  const float* hit_prob;     /* [rn,dn]: the pass' hit_prob output */
+  float* view_colors;        /* [rn,rfn,3] */
+} NrColorParams;
+int nr_view_colors(const NrPassParams* p, const NrColorParams* c, void* stream);
 
 /* Only the point kernel / only the ray kernel (profiling and stage-level tests). */
 int nr_point_kernel(const NrPassParams* p, void* stream);

@@ -65,6 +65,10 @@ class NrViewParams(C.Structure):
                 ("neuray_weights", C.c_void_p), ("geometry_weights", C.c_void_p)]
 
 
+class NrColorParams(C.Structure):
+    _fields_ = [("row_blend", C.c_void_p), ("hit_prob", C.c_void_p), ("view_colors", C.c_void_p)]
+
+
 class NrLinear(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p)]
 
@@ -102,6 +106,7 @@ SIGNATURES = {
     "nr_render_pass_fwd_tf32_agg": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrAggParams), _vp]),
     "nr_render_pass_fwd_view": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrViewParams), _vp]),
     "nr_render_pass_fwd_tf32_view": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrViewParams), _vp]),
+    "nr_view_colors": (C.c_int, [C.POINTER(NrPassParams), C.POINTER(NrColorParams), _vp]),
     "nr_point_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_point_kernel_tf32": (C.c_int, [C.POINTER(NrPassParams), _vp]),
     "nr_ray_kernel": (C.c_int, [C.POINTER(NrPassParams), _vp]),

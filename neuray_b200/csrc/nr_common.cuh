@@ -218,6 +218,15 @@ NR_HD float ld_ro(const float* p) {
 #endif
 }
 
+// four consecutive read-only floats (16-byte aligned on the device)
+NR_HD float4 ld_ro4(const float* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(reinterpret_cast<const float4*>(p));
+#else
+  return make_float4(p[0], p[1], p[2], p[3]);
+#endif
+}
+
 // ---- geometry of one query point (render_ops.py coords2rays / depth2points, dist_decoder.py get_near_far_points) ---------
 // Point n = ray * dn + s: its world position on ray `ray` at que_depth[n], the unit query direction (camera -> point,
 // negated) and the half widths of its bin towards the previous / next sample in normalised inverse depth.  cam: the query
@@ -306,6 +315,19 @@ NR_HD float bilinear(const float* plane, int fw, const Taps& t) {
 // of 64) with "x1 > x0" / "y1 > y0" in its two low bits
 NR_HD int tap_code(const Taps& t, int v, int fh, int fw) {
   return (((v * fh + t.y0) * fw + t.x0) << 6) | (t.x1 > t.x0 ? 1 : 0) | (t.y1 > t.y0 ? 2 : 0);
+}
+// the colour of view v at a valid projection (x, y): the reference's prj_dict['rgb'] (render_ops.py:132-139, the full-
+// resolution border taps with align_corners) from the [rfn, h, w, 4] RGB pack of NrPassParams::rgb.  The point kernel
+// blends this colour and nr_view_colors weights it, so both read it here.
+NR_HD void rgb_tap(const float* rgb, int v, float x, float y, int h, int w, float* out) {
+  const Taps rt = border_taps(x, y, h, w, h, w, true);
+  const float* base = rgb + size_t(v) * h * w * 4;
+  const float4 t00 = ld_ro4(base + (size_t(rt.y0) * w + rt.x0) * 4), t01 = ld_ro4(base + (size_t(rt.y0) * w + rt.x1) * 4);
+  const float4 t10 = ld_ro4(base + (size_t(rt.y1) * w + rt.x0) * 4), t11 = ld_ro4(base + (size_t(rt.y1) * w + rt.x1) * 4);
+  const float w00 = rt.w[0], w01 = rt.w[1], w10 = rt.w[2], w11 = rt.w[3];
+  out[0] = t00.x * w00 + t01.x * w01 + t10.x * w10 + t11.x * w11;
+  out[1] = t00.y * w00 + t01.y * w01 + t10.y * w10 + t11.y * w11;
+  out[2] = t00.z * w00 + t01.z * w01 + t10.z * w10 + t11.z * w11;
 }
 
 }  // namespace nr

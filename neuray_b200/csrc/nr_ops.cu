@@ -242,12 +242,13 @@ static int render_pass_fwd(const NrPassParams* p, float* rows, int exports, bool
   return launch_ray_kernel(p, stream);
 }
 
-// The pass with the blend-weight export on, then the reduction over its hit_prob.
+// The pass with the blend-weight export on, then the reduction over its hit_prob (skipped when b->blend_weights is NULL:
+// the exported row is then only for nr_view_colors).
 static int render_pass_fwd_blend(const NrPassParams* p, const NrBlendParams* b, bool tf32, cudaStream_t stream) {
   NR_CHECK_ARG(p != nullptr && b != nullptr, "params");
-  if (p->rn > 0) NR_CHECK_ARG(b->row_blend && b->blend_weights && p->hit_prob, "null blend workspace, blend_weights or hit_prob");
+  if (p->rn > 0) NR_CHECK_ARG(b->row_blend && (!b->blend_weights || p->hit_prob), "null blend workspace or hit_prob");
   const int rc = render_pass_fwd(p, b->row_blend, EXPORT_BLEND, tf32, stream);
-  if (rc != NR_OK) return rc;
+  if (rc != NR_OK || b->blend_weights == nullptr) return rc;
   return launch_blend_weights(p, b, p->hit_prob, stream);
 }
 

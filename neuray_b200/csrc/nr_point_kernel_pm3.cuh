@@ -698,14 +698,7 @@ __device__ __forceinline__ void point_body(const KParams& kp) {
         const Taps ft = border_taps(pj.ux, pj.uy, h, w, fh, fw, feat_align);
         tcode = tap_code(ft, v, fh, fw);
         tw[0] = ft.w[0]; tw[1] = ft.w[1]; tw[2] = ft.w[2]; tw[3] = ft.w[3];
-        const Taps rt = border_taps(pj.ux, pj.uy, h, w, h, w, true);
-        const float* __restrict__ base = pp.rgb + size_t(v) * h * w * 4;
-        const float4 t00 = ldg4(base + (size_t(rt.y0) * w + rt.x0) * 4), t01 = ldg4(base + (size_t(rt.y0) * w + rt.x1) * 4);
-        const float4 t10 = ldg4(base + (size_t(rt.y1) * w + rt.x0) * 4), t11 = ldg4(base + (size_t(rt.y1) * w + rt.x1) * 4);
-        const float w00 = rt.w[0], w01 = rt.w[1], w10 = rt.w[2], w11 = rt.w[3];
-        rgbin[0] = t00.x * w00 + t01.x * w01 + t10.x * w10 + t11.x * w11;
-        rgbin[1] = t00.y * w00 + t01.y * w01 + t10.y * w10 + t11.y * w11;
-        rgbin[2] = t00.z * w00 + t01.z * w01 + t10.z * w10 + t11.z * w11;
+        rgb_tap(pp.rgb, v, pj.ux, pj.uy, h, w, rgbin);
       }
     }
 

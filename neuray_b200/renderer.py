@@ -51,6 +51,9 @@ base_cfg = {
     # pixel's ray, alone and times the sample depth; view_depth_nr / view_hit_nr is where the view puts the surface
     # (nr_render_pass_fwd_view)
     "render_view_depth": False,
+    # each pass' view_colors_nr [1,rn,rfn,3]: the colour every working view puts into the pixel, Σ_d hit_prob · blend
+    # weight · the view's colour; Σ_v view_colors_nr = pixel_colors_nr (nr_view_colors)
+    "render_view_colors": False,
     # NeuralRayGenRenderer.default_cfg (renderer.py:256-261), read by predict_mean_for_depth_loss
     "use_depth_loss": False, "depth_loss_coords_num": 8192,
 }
@@ -293,7 +296,8 @@ class PassLaunch(NamedTuple):
     stream: int
 
 
-def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False, agg=False, view=False):
+def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_hit, tf32, blend=False, agg=False, view=False,
+                 colors=False):
     """Enqueues the two kernels of the pass pp; returns its raw outputs (ray_mask as uint8) and its PassLaunch, None when
     there are no rays.  tf32: the point kernel in TF32 mode (set_precision).  blend: the point kernel also exports its
     colour-blend weights and a reduction forms blend_weights [1,rn,rfn] (nr_render_pass_fwd_blend, _tf32_blend): Σ_d
@@ -303,7 +307,10 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     (ibrnet.py:349-350) of each view; with blend as well, the same launch forms blend_weights.  view: the point kernel
     also exports each view's masked hit probability hit_v (the reference's prj_dict['hit_prob'], renderer.py:75-82) and
     reductions form view_hit = Σ_d hit_v and view_depth = Σ_d hit_v · que_depth [1,rn,rfn] (nr_render_pass_fwd_view,
-    _tf32_view); the same launch forms whichever of the blend and agg outputs are asked for."""
+    _tf32_view); the same launch forms whichever of the blend and agg outputs are asked for.  colors: nr_view_colors runs
+    behind whichever of those launches runs (nr_render_pass_fwd_blend without its reduction when none is asked for), on
+    its blend row and hit_prob, and forms view_colors [1,rn,rfn,3] = Σ_d hit_prob · blending_weights_valid · the masked
+    prj_dict['rgb'] (ibrnet.py:366-367, render_ops.py:132-139) of each view."""
     cfg = owner.cfg
     coords = que_imgs_info["coords"]
     dev = coords.device
@@ -330,6 +337,8 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
     if view:
         out["view_hit"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
         out["view_depth"] = torch.empty(1, rn, pack.rfn, dtype=torch.float32, device=dev)
+    if colors:
+        out["view_colors"] = torch.empty(1, rn, pack.rfn, 3, dtype=torch.float32, device=dev)
     rec = _lib.workspace("point_rec", rn * dn * _lib.NR_POINT_REC, dev)
     p = _lib.NrPassParams()
     p.coords, p.que_depth, p.que_cam = _lib.ptr(coords_c), _lib.ptr(que_depth), _lib.ptr(cam)
@@ -360,7 +369,8 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             if _lib.PROFILE is not None:
                 raise _lib.NeurayB200Error("the point kernel is timed alone only without render_view_depth")
             w = _lib.NrViewParams()
-            w.rows = _lib.ptr(_lib.workspace("row_view", 4 * pack.rfn * rn * dn, dev))
+            rows = _lib.workspace("row_view", 4 * pack.rfn * rn * dn, dev)
+            w.rows = _lib.ptr(rows)
             w.view_hit, w.view_depth = _lib.ptr(out["view_hit"]), _lib.ptr(out["view_depth"])
             w.blend_weights = _lib.ptr(out.get("blend_weights"))
             w.neuray_weights, w.geometry_weights = _lib.ptr(out.get("neuray_weights")), _lib.ptr(out.get("geometry_weights"))
@@ -370,17 +380,19 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             if _lib.PROFILE is not None:
                 raise _lib.NeurayB200Error("the point kernel is timed alone only without render_agg_weights")
             a = _lib.NrAggParams()
-            a.rows = _lib.ptr(_lib.workspace("row_agg", 3 * pack.rfn * rn * dn, dev))
+            rows = _lib.workspace("row_agg", 3 * pack.rfn * rn * dn, dev)
+            a.rows = _lib.ptr(rows)
             a.neuray_weights, a.geometry_weights = _lib.ptr(out["neuray_weights"]), _lib.ptr(out["geometry_weights"])
             a.blend_weights = _lib.ptr(out.get("blend_weights"))
             entry = "nr_render_pass_fwd_tf32_agg" if tf32 else "nr_render_pass_fwd_agg"
             _lib.check(getattr(_lib.lib(), entry)(C.byref(p), C.byref(a), stream), entry)
-        elif blend:
+        elif blend or colors:
             if _lib.PROFILE is not None:
-                raise _lib.NeurayB200Error("the point kernel is timed alone only without render_blend_weights")
+                raise _lib.NeurayB200Error("the point kernel is timed alone only without render_blend_weights and render_view_colors")
             b = _lib.NrBlendParams()
-            b.row_blend = _lib.ptr(_lib.workspace("row_blend", pack.rfn * rn * dn, dev))
-            b.blend_weights = _lib.ptr(out["blend_weights"])
+            rows = _lib.workspace("row_blend", pack.rfn * rn * dn, dev)
+            b.row_blend = _lib.ptr(rows)
+            b.blend_weights = _lib.ptr(out.get("blend_weights"))   # NULL with colors alone: the reduction is skipped
             entry = "nr_render_pass_fwd_tf32_blend" if tf32 else "nr_render_pass_fwd_blend"
             _lib.check(getattr(_lib.lib(), entry)(C.byref(p), C.byref(b), stream), entry)
         elif _lib.PROFILE is not None:
@@ -399,7 +411,11 @@ def _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine, want_
             _lib.check(_lib.lib().nr_render_pass_fwd_tf32(C.byref(p), stream), "nr_render_pass_fwd_tf32")
         else:
             _lib.check(_lib.lib().nr_render_pass_fwd(C.byref(p), stream), "nr_render_pass_fwd")
-    _lib.count_launches(2 + (2 if view else 0) + (2 if agg else 0) + (1 if blend else 0))
+        if colors:       # plane 0 of each export workspace is the blend row
+            c = _lib.NrColorParams()
+            c.row_blend, c.hit_prob, c.view_colors = _lib.ptr(rows), _lib.ptr(out["hit_prob"]), _lib.ptr(out["view_colors"])
+            _lib.check(_lib.lib().nr_view_colors(C.byref(p), C.byref(c), stream), "nr_view_colors")
+    _lib.count_launches(2 + (2 if view else 0) + (2 if agg else 0) + (1 if blend else 0) + (1 if colors else 0))
     return out, PassLaunch(p, (coords_c, que_depth, cam, pack, w_point, w_ray, pos_enc, w_tc), (pack.rfn, pack.fh, pack.fw, 64), stream)
 
 
@@ -409,8 +425,9 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     ray_mask [1,rn] (bool), optionally fine_depth [1,rn,M], with cfg use_dr_prediction, pixel_colors_dr [1,rn,3] and
     hit_prob_dr [1,rn,dn] (direct rendering, forward only: under autograd their backward raises), with cfg
     render_visibility, visibility [1,rn,rfn], with cfg render_blend_weights, blend_weights [1,rn,rfn] and, with cfg
-    render_agg_weights, neuray_weights and geometry_weights [1,rn,rfn] and, with cfg render_view_depth, view_hit and
-    view_depth [1,rn,rfn] (none of these has a gradient: requires_grad is False).
+    render_agg_weights, neuray_weights and geometry_weights [1,rn,rfn], with cfg render_view_depth, view_hit and
+    view_depth [1,rn,rfn] and, with cfg render_view_colors, view_colors [1,rn,rfn,3] (none of these has a gradient:
+    requires_grad is False).
 
     When gradients are being recorded and the reference feature maps or any parameter of the pass require them, the
     outputs are attached to autograd through backward.RenderPassFn (forward values still come from the kernels), and the
@@ -428,10 +445,10 @@ def run_pass(owner, que_depth, que_imgs_info, ref_imgs_info, is_fine, fine=None,
     needs_grad = torch.is_grad_enabled() and (rf.requires_grad or imf.requires_grad or any(v.requires_grad for v in params))
     want_dr, want_vis = owner.cfg["use_dr_prediction"], owner.cfg.get("render_visibility", False)
     want_blend, want_agg = owner.cfg.get("render_blend_weights", False), owner.cfg.get("render_agg_weights", False)
-    want_view = owner.cfg.get("render_view_depth", False)
+    want_view, want_colors = owner.cfg.get("render_view_depth", False), owner.cfg.get("render_view_colors", False)
     out, launch = _launch_pass(owner, que_depth, que_imgs_info, ref_imgs_info, pp, fine,
-                               want_hit or want_vis or want_blend or want_agg, PRECISION == "tf32" and not needs_grad,
-                               want_blend, want_agg, want_view)
+                               want_hit or want_vis or want_blend or want_agg or want_colors, PRECISION == "tf32" and not needs_grad,
+                               want_blend, want_agg, want_view, want_colors)
     dr = _direct_render(owner, launch, rn, dn, coords.device) if want_dr else None
     if want_vis:
         out["visibility"] = _view_visibility(launch, out["hit_prob"], rn, rf.shape[0], coords.device)
@@ -454,7 +471,8 @@ _OPTIONAL_OUTPUTS = (("use_dr_prediction", "pixel_colors_dr", "pixel_colors_dr")
                      ("render_visibility", "visibility", "visibility_nr"), ("render_blend_weights", "blend_weights", "blend_weights_nr"),
                      ("render_agg_weights", "neuray_weights", "neuray_weights_nr"),
                      ("render_agg_weights", "geometry_weights", "geometry_weights_nr"),
-                     ("render_view_depth", "view_hit", "view_hit_nr"), ("render_view_depth", "view_depth", "view_depth_nr"))
+                     ("render_view_depth", "view_hit", "view_hit_nr"), ("render_view_depth", "view_depth", "view_depth_nr"),
+                     ("render_view_colors", "view_colors", "view_colors_nr"))
 
 
 def _finish_outputs(owner, res, que_imgs_info):

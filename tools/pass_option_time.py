@@ -10,13 +10,17 @@ render after warm-up.
     agg         black_800 and fern_high: cfg render_agg_weights off, on, and on together with render_blend_weights
     view        black_800 and fern_high: cfg render_view_depth off, on, and on together with render_agg_weights and
                 render_blend_weights
+    colors      black_800 and fern_high: cfg render_view_colors off, on, and on together with render_view_depth,
+                render_agg_weights and render_blend_weights
 
 Prints one JSON line: the card name, power limit and SM clocks read in the same run; per workload and arm the median
 frame time and ray-samples/s with their ranges; and the option's summary (dr_cost_ms, speedup_median and
 max_abs_diff_pixel_colors_nr_fine, visibility_cost_ms_median, blend_cost_ms_median, agg_cost_ms_median with
-agg_blend_cost_ms_median, view_cost_ms_median with view_agg_blend_cost_ms_median).  With --point-kernel, _lib.PROFILE also
-times the point kernel alone (events around each point-kernel launch); the blend, agg and view exports have no such timing.
-usage: python tools/pass_option_time.py {dr,tf32,visibility,blend,agg,view} [frames] [--point-kernel]"""
+agg_blend_cost_ms_median, view_cost_ms_median with view_agg_blend_cost_ms_median, colors_cost_ms_median with
+colors_all_cost_ms_median and all_cost_ms_median, the cost of the three other exports alone).  With --point-kernel,
+_lib.PROFILE also times the point kernel alone (events around each point-kernel launch); the blend, agg and view exports
+and the per-view colours have no such timing.
+usage: python tools/pass_option_time.py {dr,tf32,visibility,blend,agg,view,colors} [frames] [--point-kernel]"""
 import argparse
 import json
 import os
@@ -74,6 +78,16 @@ def view_summary(entry, outs):
             "view_agg_blend_cost_ms_median": round(entry["on_agg_blend"]["frame_ms"]["median"] - off, 1)}
 
 
+def colors_summary(entry, outs):
+    for arm in ("on", "on_all"):
+        assert finite(*(outs[arm]["view_colors_nr" + sfx] for sfx in ("", "_fine")))
+    off = entry["off"]["frame_ms"]["median"]
+    return {"colors_cost_ms_median": round(entry["on"]["frame_ms"]["median"] - off, 1),
+            "colors_all_cost_ms_median": round(entry["on_all"]["frame_ms"]["median"] - off, 1),
+            "all_cost_ms_median": round(entry["all"]["frame_ms"]["median"] - off, 1)}
+
+
+_ALL = {"render_view_depth": True, "render_agg_weights": True, "render_blend_weights": True}
 # option -> (workloads, {arm: (cfg overrides, render precision)}, summary)
 OPTIONS = {
     "dr": (("black_800",), {"dr_off": ({}, "fp32"), "dr_sh": ({"use_dr_prediction": True}, "fp32"),
@@ -86,6 +100,9 @@ OPTIONS = {
     "view": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_view_depth": True}, "fp32"),
                                           "on_agg_blend": ({"render_view_depth": True, "render_agg_weights": True,
                                                             "render_blend_weights": True}, "fp32")}, view_summary),
+    "colors": (("black_800", "fern_high"), {"off": ({}, "fp32"), "on": ({"render_view_colors": True}, "fp32"),
+                                            "all": (_ALL, "fp32"), "on_all": (dict(_ALL, render_view_colors=True), "fp32")},
+               colors_summary),
 }
 
 ap = argparse.ArgumentParser(description="per-frame cost of a render-pass option")
@@ -93,7 +110,7 @@ ap.add_argument("option", choices=OPTIONS)
 ap.add_argument("frames", nargs="?", type=int, default=5)
 ap.add_argument("--point-kernel", action="store_true", help="also time the point kernel alone")
 args = ap.parse_args()
-if args.option in ("blend", "agg", "view") and args.point_kernel:
+if args.option in ("blend", "agg", "view", "colors") and args.point_kernel:
     ap.error(f"the point kernel with the {args.option} export is not timed alone")
 assert torch.cuda.is_available(), "pass_option_time.py measures on a GPU"
 dev = torch.device("cuda")
